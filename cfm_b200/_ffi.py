@@ -42,7 +42,6 @@ SIGNATURES = {
     "cfm_launch_count": (C.c_longlong, []),
     "cfm_sqdist_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "cfm_sqdist_f32": (_i, [_p, _p, _p, _i, _i, _i, _i64, _i, _p, _i, _p, _sz, _p]),
-    "cfm_tc_debug_buffer": (_i, [_p]),
     "cfm_sinkhorn_workspace_bytes": (_sz, [_i, _i]),
     "cfm_sinkhorn_log_f32": (_i, [_p, _i, _i, _i64, _f, _p, _i, _i, _d, _i, _i, _d, _p, _p, _p, _p,
                                   _p, _sz, _p]),

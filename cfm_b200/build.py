@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcfm_b200.so")
-SOURCES = ["api.cu", "sqdist.cu", "sqdist_tc.cu", "sqdist_h3.cu", "sinkhorn.cu", "sinkhorn_v2.cu", "sample.cu", "assign.cu",
+SOURCES = ["api.cu", "sqdist.cu", "sqdist_h3.cu", "sinkhorn.cu", "sinkhorn_v2.cu", "sample.cu", "assign.cu",
            "gather.cu", "flow.cu", "mlp.cu", "mlp_h3.cu", "rk.cu", "ode_small.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -19,8 +19,6 @@
 // (warp shuffles + one smem hop).  No host round trips: sigma stays on the device for the
 // sampling kernel.
 #include <float.h>
-#include <stdio.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -503,9 +501,7 @@ extern "C" int cfm_assign_exact_f32(const float* M, int n, int64_t ldm, const fl
   p.g_row4col = reinterpret_cast<int32_t*>(w); w += a4;
   p.g_srlist = reinterpret_cast<int32_t*>(w); w += a4;
   p.g_sc = reinterpret_cast<unsigned char*>(w);
-  static int force_block = -1;  // CFM_ASSIGN_BLOCK=1: always use the block-wide kernel (A/B timing, tests)
-  if (force_block < 0) { const char* e = getenv("CFM_ASSIGN_BLOCK"); force_block = e ? atoi(e) : 0; }
-  if (n <= 4096 && !force_block) {
+  if (n <= 4096) {
     size_t sb = asg_fast_smem_bytes(n);
     {
       const size_t room = (size_t)200 * 1024 > sb ? (size_t)200 * 1024 - sb : 0;

@@ -91,12 +91,6 @@ __device__ __forceinline__ double warp_max(double v) {
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-// TF32 operand split for the 3xTF32 tensor-core GEMMs: hi = x with the low 13 mantissa bits cleared
-// (exactly a TF32 number), lo = tf32(x - hi)
-__device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
-  hi = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-  lo = __uint_as_float(__float_as_uint(v - hi) & 0xffffe000u);
-}
 // atomic max for non-negative floats (bit pattern order == value order)
 __device__ __forceinline__ void atomic_max_nonneg(float* addr, float v) {
   atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));

@@ -13,7 +13,7 @@
 // 3xTF32 with truncating splits 7e-8.  Range: fp16 tops out at 65504, so producers scale rows by a power of
 // two where the data is unbounded (cost matrix: per-row scales, exact) and saturate otherwise.
 //
-// Same kernel as the 3xTF32 core (gemm_tc.cuh: TMA producer warpgroup, two consumer warpgroups issuing
+// Runs on the persistent GEMM core of gemm_tc.cuh (TMA producer warpgroup, two consumer warpgroups issuing
 // wgmma m64n128k16, 3-stage ring), with a K-chunk of 64 fp16 (= the 128-byte swizzle atom), 4 k-steps of K = 16
 // per chunk and 3 MMAs per k-step into the two accumulators (2 x 64 registers per thread: the 128 x 128 tile is
 // the largest whose two fp32 accumulators fit the register file).
@@ -67,7 +67,7 @@ __device__ __forceinline__ void split_h3_sat_x2(float v0, float v1, uint32_t& hi
 
 // ---- host side -------------------------------------------------------------------------------------
 // (rows, d) fp16 row-major (row stride ld halves, ld % 8 == 0) -> box of (box_rows x 64 halves), 128B swizzle,
-// zero fill outside [0, d) x [0, rows).  Descriptors are cached by (base, shape): see sqdist_tc.cu.
+// zero fill outside [0, d) x [0, rows).  Descriptors are cached by (base, shape): see sqdist_h3.cu.
 int tc_make_map_f16(CUtensorMap* m, const __half* base, int rows, int d, int64_t ld, int box_rows);
 
 // Epilogue functor interface: see gemm_tc.cuh (acc = acc0 + acc1 * 2^-11)
@@ -80,7 +80,7 @@ inline int launch_gemm_h3(const __half* ah, const __half* al, int n0, int64_t ld
   if ((rc = tc_make_map_f16(&mal, al, n0, d, lda, kTM)) != CFM_OK) return rc;
   if ((rc = tc_make_map_f16(&mbh, bh, n1, d, ldb, kTN)) != CFM_OK) return rc;
   if ((rc = tc_make_map_f16(&mbl, bl, n1, d, ldb, kTN)) != CFM_OK) return rc;
-  return launch_gemm_wg<H3Scheme>(mah, mal, mbh, mbl, n0, n1, d, epi, false, s);
+  return launch_gemm_wg<H3Scheme>(mah, mal, mbh, mbl, n0, n1, d, epi, s);
 }
 
 }  // namespace cfm

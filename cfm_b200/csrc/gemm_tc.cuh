@@ -1,10 +1,6 @@
-// Reusable Hopper tensor-core GEMM core:  D[m, n] = sum_k A[m, k] * B[n, k]  at fp32-grade accuracy.
-// Two operand schemes share one kernel (gemm_wg_kernel, parameterised by a Scheme type):
-//   * 3xTF32 (this file, TfScheme): A = A_hi + A_lo, B = B_hi + B_lo, all four K-major fp32 arrays whose entries are
-//     exactly TF32 numbers;  D ~= A_lo.B_hi + A_hi.B_lo + A_hi.B_hi  accumulated in ONE fp32 register accumulator
-//     (wgmma ... .tf32).  The tensor core's accumulator truncates at each of the 3*K/8 accumulate steps, so the result
-//     is good to ~1e-6 of sum|a||b| (fp32 FMA: ~1e-7).
-//   * fp16x3 (gemm_h3.cuh, H3Scheme): two accumulators, see there.
+// Reusable Hopper tensor-core GEMM core:  D[m, n] = sum_k A[m, k] * B[n, k]  at fp32-grade accuracy, with each
+// operand carried as a (hi, lo) pair.  The kernel (gemm_wg_kernel) is parameterised by a Scheme type that fixes the
+// element type, the K-chunk and the MMAs of one k-step: the fp16x3 scheme (gemm_h3.cuh, H3Scheme).
 //
 // Persistent warp-specialised kernel, one CTA per SM, 384 threads = three warpgroups:
 //   warpgroup 0      TMA producer (one thread): 4 tiled loads per K-chunk (A_hi, A_lo: 128 rows; B_hi, B_lo: 128
@@ -20,12 +16,10 @@
 //                    -- store32 is called by the whole warp, which writes the chunk coalesced via tc_store_chunk32.
 //                    Meanwhile the producer already streams the next tile's stages.
 // Tiles are walked M-fastest so the B panel stays hot in L2.
-// Users: sqdist_tc.cu (cost matrix, algo 2: round 1's 3xTF32 path, kept for A/B) and, through gemm_h3.cuh, the
-// fp16x3 cost matrix and the per-layer MLP.  The PTX wrappers below are shared with mlp_h3.cu's fused kernel.
+// Users, through gemm_h3.cuh: the fp16x3 cost matrix and the per-layer MLP.  The PTX wrappers below are shared with
+// mlp_h3.cu's fused kernel.
 #pragma once
 #include <cuda.h>
-#include <stdlib.h>
-#include <string.h>
 
 #include "common.cuh"
 
@@ -38,19 +32,11 @@ constexpr int kWgStageBytes = 4 * kTileBytes;              // A_hi | A_lo | B_hi
 constexpr int kWgStagingBytes = 2 * 64 * 64 * 4;           // per consumer warpgroup: 64 rows x 64 fp32 columns
 constexpr size_t kWgSmemBytes = (size_t)kWgStages * kWgStageBytes + kWgStagingBytes + 256;
 constexpr int kWgThreads = 384;
-constexpr int kTK = 32;  // fp32 K-chunk (32 fp32 = 128 B swizzle atom)
 
 struct TcShape {
   int n0, n1, d;          // rows of A, rows of B (= output columns), K
   int tiles_m, tiles_n;
-  unsigned long long* dbg;  // optional: 8 globaltimer checkpoints per CTA (CFM_TC_DEBUG), else null
 };
-__device__ __forceinline__ unsigned long long tc_now() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define TC_MARK(slot) do { if (p.dbg) p.dbg[blockIdx.x * 8 + (slot)] = tc_now(); } while (0)
 
 // ---- PTX wrappers --------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -130,14 +116,6 @@ __device__ __forceinline__ void wg_mma_f16_n128(float (&d)[64], uint64_t adesc, 
       : CFM_WG_ACC64(d)
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// d[64] (+)= A(64 x 8 tf32) . B(128 x 8 tf32)^T, both K-major in shared memory
-__device__ __forceinline__ void wg_mma_tf32_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " CFM_WG_REGS64 ", %64, %65, p, 1, 1;\n\t}\n"
-      : CFM_WG_ACC64(d)
-      : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
 
 // Accumulator fragment of wgmma m64nN (fp32): thread (warp w of the warpgroup, lane l) holds, for every 8-column
 // group i, rows 16w + l/4 and 16w + l/4 + 8 at columns 8i + 2(l%4) + {0, 1}:  d[4i + {0,1}] and d[4i + {2,3}].
@@ -164,18 +142,6 @@ __device__ __forceinline__ void tc_store_chunk32(float* tile, const float (&v)[3
   __syncwarp();
 }
 
-// 3xTF32 scheme: one accumulator, three MMAs per k-step of 8 (small terms first)
-struct TfScheme {
-  static constexpr int kElem = 4, kKChunk = 32, kKStep = 8, kNAcc = 1;
-  __device__ static __forceinline__ void mma(float (&d0)[64], float (&)[64], uint64_t ah, uint64_t al, uint64_t bh,
-                                             uint64_t bl, uint32_t first) {
-    wg_mma_tf32_n128(d0, al, bh, first);
-    wg_mma_tf32_n128(d0, ah, bl, 1u);
-    wg_mma_tf32_n128(d0, ah, bh, 1u);
-  }
-  __device__ static __forceinline__ float combine(float a0, float) { return a0; }
-};
-
 template <class Scheme, class Epi>
 __global__ void __launch_bounds__(kWgThreads, 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
@@ -189,7 +155,6 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   uint64_t* empty = full + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) TC_MARK(0);  // kernel entry
   const int num_tiles = p.tiles_m * p.tiles_n;
   const int nk = (p.d + kK - 1) / kK;
 
@@ -198,11 +163,6 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  // Programmatic dependent launch: everything above touches no memory written by the preceding kernel, so when
-  // this grid is launched with the programmatic-serialization attribute its prologue overlaps the tail of its
-  // predecessor; from here on the predecessor's results are needed.  Without the attribute both are no-ops.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   if (warp < 4) {
     // ===================== TMA producer =====================
@@ -292,26 +252,18 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
       }
     }
     epi.finish(lane);
-    if (threadIdx.x == 128) TC_MARK(5);  // all epilogues of this CTA done
   }
 }
 
 // ---- host side -------------------------------------------------------------------------------------
-// (rows, d) fp32 row-major (row stride ld floats) -> box of (box_rows x 32 floats), 128B swizzle, zero OOB fill
-int tc_make_map(CUtensorMap* m, const float* base, int rows, int d, int64_t ld, int box_rows);
-unsigned long long* tc_debug_buffer();  // device buffer set through cfm_tc_debug_buffer(), else null
-// x -> (hi, lo) TF32 split of n contiguous floats (sqdist_tc.cu)
-int tc_split(const float* x, float* hi, float* lo, int64_t n, cudaStream_t s);
-
 // launch of gemm_wg_kernel on prepared tensor maps (grid = min(tiles, SMs))
 template <class Scheme, class Epi>
 inline int launch_gemm_wg(const CUtensorMap& mah, const CUtensorMap& mal, const CUtensorMap& mbh,
-                          const CUtensorMap& mbl, int n0, int n1, int d, Epi epi, bool pdl, cudaStream_t s) {
+                          const CUtensorMap& mbl, int n0, int n1, int d, Epi epi, cudaStream_t s) {
   TcShape p;
   p.n0 = n0; p.n1 = n1; p.d = d;
   p.tiles_m = (n0 + kTM - 1) / kTM;
   p.tiles_n = (n1 + kTN - 1) / kTN;
-  p.dbg = tc_debug_buffer();
   auto kern = gemm_wg_kernel<Scheme, Epi>;
   static bool attr_set = false;  // per (Scheme, Epi) instantiation
   if (!attr_set) {
@@ -320,35 +272,10 @@ inline int launch_gemm_wg(const CUtensorMap& mah, const CUtensorMap& mal, const 
   }
   int grid = p.tiles_m * p.tiles_n;
   if (grid > sm_count()) grid = sm_count();
-  if (pdl) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kWgThreads); cfg.dynamicSmemBytes = kWgSmemBytes; cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    CFM_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mah, mal, mbh, mbl, p, epi));
-  } else {
-    kern<<<grid, kWgThreads, kWgSmemBytes, s>>>(mah, mal, mbh, mbl, p, epi);
-  }
+  kern<<<grid, kWgThreads, kWgSmemBytes, s>>>(mah, mal, mbh, mbl, p, epi);
   ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
-}
-
-template <class Epi>
-inline int launch_gemm_tc(const float* ah, const float* al, int n0, int64_t lda, const float* bh,
-                          const float* bl, int n1, int64_t ldb, int d, Epi epi, cudaStream_t s) {
-  CUtensorMap mah, mal, mbh, mbl;
-  int rc;
-  if ((rc = tc_make_map(&mah, ah, n0, d, lda, kTM)) != CFM_OK) return rc;
-  if ((rc = tc_make_map(&mal, al, n0, d, lda, kTM)) != CFM_OK) return rc;
-  if ((rc = tc_make_map(&mbh, bh, n1, d, ldb, kTN)) != CFM_OK) return rc;
-  if ((rc = tc_make_map(&mbl, bl, n1, d, ldb, kTN)) != CFM_OK) return rc;
-  static int pdl = -1;  // CFM_TC_PDL=1: launch as a programmatic dependent of the preceding kernel in the stream
-  if (pdl < 0) { const char* e = getenv("CFM_TC_PDL"); pdl = e ? atoi(e) : 0; }
-  return launch_gemm_wg<TfScheme>(mah, mal, mbh, mbl, n0, n1, d, epi, pdl != 0, s);
 }
 
 }  // namespace cfm

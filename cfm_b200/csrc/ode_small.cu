@@ -28,8 +28,6 @@
 // met behind 128-thread named barriers: 5x fewer instructions per warp, but four barriers per evaluation and the
 // Runge-Kutta arithmetic of a 2-D state serialised in one warp ate the gain).
 #include <cooperative_groups.h>
-#include <stdio.h>
-#include <stdlib.h>
 
 #include "mlp_common.cuh"
 
@@ -68,7 +66,6 @@ struct OdeSmallParams {
   double* partials;  // [2][3][gridDim.x]
   int rows_per_warp;
   int max_steps;
-  int dbg;  // CFM_ODE_DBG=1: CTA 0 prints its clock64 breakdown (debugging aid)
 };
 
 constexpr int kSlots = 9;  // x, k1..k7, xnew
@@ -419,11 +416,8 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
   }
 
   int steps = 0;
-  long long c_eval = 0, c_sum = 0, c_ctl = 0, c_mlp = 0;
-  const long long c_begin = clock64();
   while (!done && steps < p.max_steps) {
     ++steps;
-    long long c0 = clock64();
     double es[1] = {0.0};
     for (int g = 0; g < rpw; g += RB) {
       if (row_of(g) >= B) break;
@@ -447,10 +441,8 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
           }
         }
         __syncwarp();
-        const long long m0 = clock64();
         mlp_eval<U>(sm, pl, dim, tv, act, d0p, d1p, t + oC[stage] * dt, hA, hB, slot(g, 1 + stage),
                     slot(g + 1, 1 + stage), lane);
-        c_mlp += clock64() - m0;
       }
 #pragma unroll
       for (int m = 0; m < RB; ++m) {
@@ -468,12 +460,8 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
         }
       }
     }
-    long long c1 = clock64();
-    c_eval += c1 - c0;
     grid_sum<1>(grid, es, p.partials, pbuf, red);
     pbuf ^= 1;
-    c0 = clock64();
-    c_sum += c0 - c1;
     // ---- controller (rk.cu rk_control_kernel, torchdyn order) ----
     ratio = (float)sqrt(es[0] / numel);
     nfe += 6;
@@ -516,11 +504,7 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
       }
       __syncwarp();
     }
-    c_ctl += clock64() - c0;
   }
-  if (p.dbg && blockIdx.x == 0 && tid == 0)
-    printf("ode_small: steps %d  cycles total %lld  stages+evals %lld (mlp %lld)  grid_sum %lld  control+commit %lld\n",
-           steps, clock64() - c_begin, c_eval, c_mlp, c_sum, c_ctl);
   if (blockIdx.x == 0 && tid == 0) {
     cfm_rk_state* st = p.st;
     st->t = t; st->dt = dt; st->t_end = t_end; st->atol = atol; st->rtol = rtol;
@@ -618,7 +602,6 @@ extern "C" int cfm_ode_small_trajectory_f32(const float* W0, const float* b0, co
   p.x0 = x0; p.B = batch; p.t_span = t_span; p.n_span = n_span; p.atol = atol; p.rtol = rtol;
   p.solver = solver; p.traj = traj; p.st = state_out; p.partials = reinterpret_cast<double*>(workspace);
   p.rows_per_warp = L.rpw; p.max_steps = 1000000;
-  { const char* e = getenv("CFM_ODE_DBG"); p.dbg = e ? atoi(e) : 0; }
   cudaStream_t s = (cudaStream_t)stream;
   CFM_CUDA_OK(cudaMemsetAsync(state_out, 0, sizeof(cfm_rk_state), s));
   if (w == 32) return launch<1>(p, L, s);

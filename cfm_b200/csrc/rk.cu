@@ -32,9 +32,9 @@ __constant__ float kA[7][6] = CFM_RK_A_INIT;
 // b5 - b4 (embedded error weights), k1..k7
 __constant__ float kE[7] = CFM_RK_E_INIT;
 
-// L2 policies for the stage-input reads (CFM_RK_L2 bitmask, read once): a dopri5 step re-reads x and k1 in every one of
-// its six stage inputs while ~1 GB of other traffic (2.5x the L2) passes in between; loading them evict_last keeps
-// them resident.  bit 0: x evict_last, bit 1: k1 evict_last, bit 2: k2..k6 evict_first.
+// L2 policies for the stage-input reads: a dopri5 step re-reads x and k1 in every one of its six stage inputs while
+// ~1 GB of other traffic (2.5x the L2) passes in between; loading them evict_last keeps them resident.  k2..k6 are
+// loaded evict_first.
 __device__ __forceinline__ uint64_t rk_policy(bool last) {
   uint64_t p;
   if (last) asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
@@ -47,11 +47,6 @@ __device__ __forceinline__ float4 rk_ld_pol(const float4* ptr, uint64_t pol) {
       : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(ptr), "l"(pol));
   return v;
 }
-static int rk_l2_mode() {
-  static int m = -1;
-  if (m < 0) { const char* e = getenv("CFM_RK_L2"); m = e ? atoi(e) : 7; }
-  return m;
-}
 
 static inline int ew_grid(int64_t numel) {
   int64_t blocks = (numel / 4 + 255) / 256 + 1;
@@ -59,11 +54,9 @@ static inline int ew_grid(int64_t numel) {
   return (int)(blocks < cap ? blocks : cap);
 }
 
-static inline int rk_stage_grid(int64_t numel) {  // CFM_RK_GRID: CTAs per SM of the stage-input kernel (default 8)
-  static int per_sm = -1;
-  if (per_sm < 0) { const char* e = getenv("CFM_RK_GRID"); per_sm = e ? atoi(e) : 8; }
+static inline int rk_stage_grid(int64_t numel) {  // at most 8 CTAs per SM
   int64_t blocks = (numel / 8 + 255) / 256 + 1;
-  const int64_t cap = (int64_t)sm_count() * per_sm;
+  const int64_t cap = (int64_t)sm_count() * 8;
   return (int)(blocks < cap ? blocks : cap);
 }
 
@@ -87,8 +80,8 @@ __host__ __device__ constexpr float rk_e(int j) { constexpr float t[7] = CFM_RK_
 // xs (stage 1..5) or xnew (stage 6) = x + dt * sum_j a[stage][j] * k_j ; also t_stage = t + c*dt.
 // STAGE is a template parameter so that the loads of a thread -- x and the stage's derivative arrays, for U float4
 // positions -- are straight-line code issued back to back (up to 12 independent 128-bit loads in flight per thread);
-// L2MODE: see rk_policy above.
-template <int STAGE, int L2MODE>
+// L2 policies: see rk_policy above.
+template <int STAGE>
 __global__ void __launch_bounds__(256)
 rk_stage_input_kernel(const cfm_rk_state* __restrict__ st, const float* __restrict__ x,
                       const float* __restrict__ k, float* __restrict__ out,
@@ -96,7 +89,6 @@ rk_stage_input_kernel(const cfm_rk_state* __restrict__ st, const float* __restri
                       float* __restrict__ t_stage, float* __restrict__ err_partial, int64_t numel) {
   if (st->done) return;
   constexpr int stage = STAGE;
-  constexpr int l2mode = L2MODE;
   constexpr int U = 2;
   const float dt = st->dt;
   const uint64_t pol_last = rk_policy(true), pol_first = rk_policy(false);
@@ -111,14 +103,12 @@ rk_stage_input_kernel(const cfm_rk_state* __restrict__ st, const float* __restri
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int64_t i = i0 + u * stride < n4 ? i0 + u * stride : i0;  // (a clamped duplicate instead of a branch)
-      v[u] = (l2mode & 1) ? rk_ld_pol(reinterpret_cast<const float4*>(x) + i, pol_last)
-                          : __ldg(reinterpret_cast<const float4*>(x) + i);
+      v[u] = rk_ld_pol(reinterpret_cast<const float4*>(x) + i, pol_last);
 #pragma unroll
       for (int j = 0; j < 6; ++j)
         if (j < stage && rk_a(stage, j) != 0.f) {
           const float4* kp = reinterpret_cast<const float4*>(k + (int64_t)j * numel) + i;
-          kk[u][j] = (j == 0 && (l2mode & 2)) ? rk_ld_pol(kp, pol_last)
-                     : (j > 0 && (l2mode & 4)) ? rk_ld_pol(kp, pol_first) : __ldg(kp);
+          kk[u][j] = rk_ld_pol(kp, j == 0 ? pol_last : pol_first);
         }
     }
 #pragma unroll
@@ -440,12 +430,9 @@ extern "C" int cfm_rk_stage_input(const cfm_rk_state* st, const float* x, const 
              reinterpret_cast<uintptr_t>(out_hi) | reinterpret_cast<uintptr_t>(out_lo)) & 15) == 0);
   RK_CHECK(err_partial == nullptr || stage == 6);
   using Kern = void (*)(const cfm_rk_state*, const float*, const float*, float*, __half*, __half*, float*, float*, int64_t);
-#define CFM_RK_ROW(M) {rk_stage_input_kernel<1, M>, rk_stage_input_kernel<2, M>, rk_stage_input_kernel<3, M>, \
-                       rk_stage_input_kernel<4, M>, rk_stage_input_kernel<5, M>, rk_stage_input_kernel<6, M>}
-  static const Kern table[4][6] = {CFM_RK_ROW(0), CFM_RK_ROW(3), CFM_RK_ROW(4), CFM_RK_ROW(7)};
-#undef CFM_RK_ROW
-  const int m = rk_l2_mode();
-  const Kern kern = table[m == 3 ? 1 : m == 4 ? 2 : m == 7 ? 3 : 0][stage - 1];
+  static const Kern table[6] = {rk_stage_input_kernel<1>, rk_stage_input_kernel<2>, rk_stage_input_kernel<3>,
+                                rk_stage_input_kernel<4>, rk_stage_input_kernel<5>, rk_stage_input_kernel<6>};
+  const Kern kern = table[stage - 1];
   kern<<<rk_stage_grid(numel), 256, 0, (cudaStream_t)stream>>>(
       st, x, k, out, reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo), t_stage, err_partial, numel);
   ::cfm::note_launches(1);

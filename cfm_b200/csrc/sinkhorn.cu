@@ -898,7 +898,7 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
     SK_TL(1);
     const float dv_min = it > 0 ? global_min(dmin_v) : 0.f;
     SK_TL(2);
-    const bool fused = it > 0 && do_col && p.screen_fused;
+    const bool fused = it > 0 && do_col;
     if (!fused) {
       row_phase(it > 0, dv_min);
       SK_TL(3);
@@ -1083,12 +1083,10 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
   }
   // precise: -1 auto, 0 fp32, 1 float64, 2 fp32 on the generic kernel, 3 float64 with fp32 exponentials ("mixed"),
   // 4 = 3 without the screening of negligible terms
-  static int auto_mixed = -1;  // CFM_SK_MIXED: what auto mode uses when it needs float64 potentials
-  if (auto_mixed < 0) { const char* e = getenv("CFM_SK_MIXED"); auto_mixed = e ? atoi(e) : 1; }  // 1: "mixed" (fp32 exponentials of float64 differences)
-  int screen_off = 0;
-  if (precise == 4) { precise = 3; screen_off = 1; }  // mixed without the fp32 screening (cross-checks, A/B)
+  p.screen = 1;
+  if (precise == 4) { precise = 3; p.screen = 0; }  // mixed without the fp32 screening (cross-checks)
   if (precise == 3) { precise = 1; p.precise = 1; p.mixed = 1; }
-  else if (precise < 0) p.mixed = auto_mixed;
+  else if (precise < 0) p.mixed = 1;  // auto mode needing float64 potentials: "mixed" (fp32 exponentials of float64 differences)
   // fast fp32 mode on aligned n1 <= 8192: smem-staged kernel (sinkhorn_v2.cu)
   if (precise == 2) { precise = 0; p.precise = 0; }  // fast arithmetic, generic kernel (cross-checks)
   else if (precise != 1) {
@@ -1105,12 +1103,6 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
   const size_t vbytes = (size_t)p.n1p * 12;  // float64 stage + its fp32 copy (screened mixed mode)
   p.v_in_smem = vbytes <= 160 * 1024;
   const size_t smem = p.v_in_smem ? vbytes : 0;
-  static int screen = -1;
-  if (screen < 0) { const char* e = getenv("CFM_SK_SCREEN"); screen = e ? atoi(e) : 1; }
-  p.screen = screen_off ? 0 : screen;
-  static int sfused = -1;
-  if (sfused < 0) { const char* e = getenv("CFM_SK_FUSED"); sfused = e ? atoi(e) : 1; }
-  p.screen_fused = sfused;
   static int tl = -1;
   if (tl < 0) { const char* e = getenv("CFM_SK_TL"); tl = e ? atoi(e) : 0; }
   p.timeline = tl;

@@ -41,13 +41,9 @@ struct SkParams {
   int vec;          // float4 path usable
   int v_in_smem;
   float l2_resident_frac;  // sinkhorn_v2: share of each slab loaded with L2 evict_last (0: default policy)
-  int dbg_flags;    // sinkhorn_v2 A/B switches (CFM_SK_DBG)
-  int atomic_cols;      // sinkhorn_v2, factored regime: reduce the column partials with fixed-point atomics (one barrier per sweep)
-  int prefetch_chunks;  // sinkhorn_v2: row chunks per CTA prefetched into L2 during the inter-sweep barriers
   int run_if;       // 0 always; 1 only when auto-mode resolves to fast; 2 only when it resolves to precise
   int timeline;     // seeded solver: globaltimer marks of one iteration (CFM_SK_TL; debug aid)
-  int screen_fused; // seeded screening: fused row + column sweep with an assumed bound (CFM_SK_FUSED, default 1)
-  int screen;       // mixed mode: fp32 screening of negligible terms (CFM_SK_SCREEN, default 1; 0 = round-2a path)
+  int screen;       // mixed mode: fp32 screening of negligible terms (0 only for precise = 4, the unscreened reference)
   int mixed;        // precise mode only: float64 potentials and exponent ARGUMENTS, fp32 exponentials (see expd)
 };
 

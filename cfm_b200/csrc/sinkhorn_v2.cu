@@ -29,8 +29,7 @@
 
 namespace cfm {
 
-// NT = threads per CTA (512: one CTA per SM; 256: two CTAs per SM whose barrier domains are
-// independent, so one CTA's per-chunk latency chain is hidden behind the other's work)
+// NT = threads per CTA: 512, one CTA per SM
 
 __device__ __forceinline__ uint32_t v2_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void v2_mbar_init(uint64_t* bar, uint32_t count) {
@@ -62,10 +61,6 @@ __device__ __forceinline__ void v2_bulk_load_hint(void* dst, const void* src, ui
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
                ::"r"(v2_smem_u32(dst)), "l"(src), "r"(bytes), "r"(v2_smem_u32(bar)), "l"(policy) : "memory");
 }
-// fire-and-forget L2 prefetch of a contiguous global range (no shared memory, no completion tracking)
-__device__ __forceinline__ void v2_prefetch_l2(const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ uint64_t v2_policy_evict_last() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
@@ -75,23 +70,6 @@ __device__ __forceinline__ uint64_t v2_policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
-}
-// Minimal grid barrier for the co-resident (cooperatively launched) grid: thread 0 of every CTA
-// releases its CTA's global writes, arrives with one atomic and spins with acquire loads until the
-// running counter reaches `target` (= barrier ordinal * gridDim.x).  Cheaper than
-// cooperative_groups::grid.sync() at one 512-thread CTA per SM.
-__device__ __forceinline__ void v2_grid_barrier(unsigned int* counter, unsigned int target) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    atomicAdd(counter, 1u);
-    unsigned int seen;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-    } while (seen < target);
-    __threadfence();
-  }
-  __syncthreads();
 }
 template <int NT>
 __device__ __forceinline__ void v2_consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
@@ -126,9 +104,8 @@ __device__ __forceinline__ int multi_row(int lane) {
 }
 
 template <int NT, int KG, int R>
-__global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParams p, const int S) {
+__global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, const int S) {
   constexpr int kV2Consumers = NT, kV2Threads = NT, kV2Warps = NT / 32;
-  constexpr bool kVSmem = KG > 4;  // 32 columns per thread: keep V_j in thread-private smem slots
   extern __shared__ __align__(128) unsigned char v2_smem[];
   cg::grid_group grid = cg::this_grid();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -146,7 +123,6 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
   float* stages = reinterpret_cast<float*>(v2_smem);
   float2* rowpart = reinterpret_cast<float2*>(stages + (size_t)S * stage_floats);  // [2][R][16]
   uint64_t* full = reinterpret_cast<uint64_t*>(rowpart + 2 * R * kV2Warps);
-  float* V_s = reinterpret_cast<float*>(full + 8);  // n1p floats when kVSmem
   __shared__ double red[kV2Warps];
 
   if (tid == 0) {
@@ -179,11 +155,6 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
   int p_dir = 1;              // sweeps alternate direction (boustrophedon): the rows a sweep ends on are
                               // the rows the next one starts on, and those are still resident in L2
   int sweep_no = 0;
-  unsigned int* gbar = reinterpret_cast<unsigned int*>(p.err_ring + 4);  // zeroed by the launcher
-  unsigned int gbar_n = 0;
-  // cg::grid.sync() is the iteration barrier: the hand-rolled atomic-counter v2_grid_barrier and a flag-array barrier
-  // (one word per CTA, warp 0 polling all words) are kept for A/B experiments
-  auto grid_sync = [&]() { (void)gbar; (void)gbar_n; grid.sync(); };
   long long issued = 0, consumed_total = 0;
   bool gvalid[KG];
 #pragma unroll
@@ -215,51 +186,26 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
   };
   if (tid == 0)
     for (int q = 0; q < S; ++q) issue_next();  // initial fill (wraps into the next sweep if S > nchunks)
-  // While the grid sits in the two barriers and the combine between two sweeps the HBM
-  // is idle except for the refill of the shared-memory ring (S chunks).  Thread 0 uses that window: at the end
-  // of a sweep it prefetches into L2 the p.prefetch_chunks chunks the next sweep will ask for right after the
-  // ones already in the ring, so the sweep starts on L2 hits and the DRAM transfer of those rows overlaps the
-  // barrier latency instead of the streaming phase.  A hint only: results do not depend on it.
-  auto prefetch_ahead = [&]() {
-    int c = p_chunk, dir = p_dir;
-    for (int q = 0; q < p.prefetch_chunks; ++q) {
-      if (c < 0 || c >= nchunks) break;  // the sweep after next is not worth fetching yet
-      if (!(resident >= 0 && c < resident)) {  // resident chunks are L2 hits already
-        const int r0 = r_begin + c * R;
-        const int rv = min(R, r_begin + nrows - r0);
-        for (int r = 0; r < rv; ++r) v2_prefetch_l2(p.M + (int64_t)(r0 + r) * p.ldm, (uint32_t)n1 * 4u);
-      }
-      c += dir;
-    }
-  };
 
   // ---- one fused sweep ----
-  // v_in (single-barrier mode): this thread's columns of v in registers and the common reference vref_in;
-  // acc_out (single-barrier mode): fixed-point column accumulator the partials are added to
-  // v_reload (single-barrier mode): where this thread parked its v before the sweep (re-read for the partial scaling
-  // at the end, so that 16 registers do not stay live across the streaming loop); null = v is zero (prologue)
-  auto sweep = [&](bool do_row, bool do_col, const float* v_cur, const float4* v_in, float vref_in,
-                   unsigned long long* acc_out, const float* v_reload) {
+  auto sweep = [&](bool do_row, bool do_col, const float* v_cur) {
     if (fact) {
       // ---------------- factored (kernel-space in registers) sweep ----------------
-      const float vref = do_row ? (v_in ? vref_in : __ldcg(v_cur)) : 0.f;
+      const float vref = do_row ? __ldcg(v_cur) : 0.f;
       const float nkap = -kappa;
-      float4 V[kVSmem ? 1 : KG];
+      float4 V[KG];
       float cs[KG][4];
 #pragma unroll
       for (int k = 0; k < KG; ++k) {
-        float4 vk = make_float4(0.f, 0.f, 0.f, 0.f);  // idle columns: weight 0
+        V[k] = make_float4(0.f, 0.f, 0.f, 0.f);  // idle columns: weight 0
         if (gvalid[k]) {
           if (do_row) {
-            const float4 vv = v_in ? v_in[k]
-                                   : __ldcg(reinterpret_cast<const float4*>(v_cur + tcol + kV2Consumers * 4 * k));
-            vk = make_float4(ex2f(vv.x - vref), ex2f(vv.y - vref), ex2f(vv.z - vref), ex2f(vv.w - vref));
+            const float4 vv = __ldcg(reinterpret_cast<const float4*>(v_cur + tcol + kV2Consumers * 4 * k));
+            V[k] = make_float4(ex2f(vv.x - vref), ex2f(vv.y - vref), ex2f(vv.z - vref), ex2f(vv.w - vref));
           } else {
-            vk = make_float4(1.f, 1.f, 1.f, 1.f);
+            V[k] = make_float4(1.f, 1.f, 1.f, 1.f);
           }
         }
-        if (kVSmem) *reinterpret_cast<float4*>(V_s + tcol + kV2Consumers * 4 * k) = vk;  // private slot
-        else V[k] = vk;
 #pragma unroll
         for (int c = 0; c < 4; ++c) cs[k][c] = 0.f;
       }
@@ -305,10 +251,8 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
             float s = 0.f;
 #pragma unroll
             for (int k = 0; k < KG; ++k) {
-              const float4 vk = kVSmem ? *reinterpret_cast<const float4*>(V_s + tcol + kV2Consumers * 4 * k)
-                                       : V[kVSmem ? 0 : k];
-              s = fmaf(E[r][k].x, vk.x, s); s = fmaf(E[r][k].y, vk.y, s);
-              s = fmaf(E[r][k].z, vk.z, s); s = fmaf(E[r][k].w, vk.w, s);
+              s = fmaf(E[r][k].x, V[k].x, s); s = fmaf(E[r][k].y, V[k].y, s);
+              s = fmaf(E[r][k].z, V[k].z, s); s = fmaf(E[r][k].w, V[k].w, s);
             }
             sr[r] = s;
           }
@@ -362,27 +306,7 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
       }
       consumed_total += nchunks;
       ++sweep_no;
-      if (tid == 0) prefetch_ahead();
-      if (do_col && acc_out != nullptr) {
-        // Single-barrier mode.  Column sum C_j = sum_b cs_bj 2^(kappa + uref_b) and v_new_j = logb - log2 C_j, so
-        // with q_bj = cs_bj 2^(kappa + uref_b + v_j - logb):  sum_b q_bj = 2^(v_j - v_new_j)  (= 1 at the fixed
-        // point).  The q's are added as 32.32 fixed-point integers: integer addition is associative, so the
-        // total -- unlike a floating-point atomic sum -- does not depend on the arrival order of the CTAs.
-        const float sh = kappa + uref - logb;
-#pragma unroll
-        for (int k = 0; k < KG; ++k)
-          if (gvalid[k]) {
-            const float4 vv = v_reload ? __ldcg(reinterpret_cast<const float4*>(v_reload + tcol + kV2Consumers * 4 * k))
-                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-            const float vq[4] = {vv.x, vv.y, vv.z, vv.w};
-            unsigned long long* dst = acc_out + tcol + kV2Consumers * 4 * k;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const float q = cs[k][c] * ex2f(sh + vq[c]) * 4294967296.f;
-              atomicAdd(dst + c, (unsigned long long)__float2ll_rn(fminf(fmaxf(q, 0.f), 4.0e18f)));
-            }
-          }
-      } else if (do_col) {
+      if (do_col) {
         // sum_i ex2(M c2 + u_i) over this slab = cs * 2^(kappa + uref): partial (max, sum) form
         const float pm = kappa + uref;
 #pragma unroll
@@ -486,7 +410,6 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
     }
     consumed_total += nchunks;
     ++sweep_no;
-    if (tid == 0) prefetch_ahead();
     if (do_col) {
 #pragma unroll
       for (int k = 0; k < KG; ++k)
@@ -510,24 +433,7 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
       const bool act = j < c_end;
       float m = -1.0e30f, s = 0.f;
       if (act) {
-        if (p.dbg_flags & 1) {  // A/B: previous 4-wide variant
-          for (int c0 = sub; c0 < nblk; c0 += 32) {
-            float mm[4], ss[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int c = c0 + q * 8;
-              if (c < nblk) {
-                mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
-                ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
-              } else { mm[q] = -1.0e30f; ss[q] = 0.f; }
-            }
-            const float bm = fmaxf(fmaxf(fmaxf(mm[0], mm[1]), fmaxf(mm[2], mm[3])), m);
-            float acc = s * ex2f(m - bm);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc += ss[q] * ex2f(mm[q] - bm);
-            s = acc; m = bm;
-          }
-        } else if (!(p.dbg_flags & 4) && nblk <= 152) {
+        if (nblk <= 152) {
           // every lane loads ALL its <= 19 (max, sum) pairs before it reduces: ONE L2 round trip per column instead of
           // three dependent ones (the combine sits between the two grid barriers: its latency is fixed cost per iteration)
           float mm[19], ss[19];
@@ -547,7 +453,7 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
           for (int q = 0; q < 19; ++q) acc += ss[q] * ex2f(mm[q] - bm);
           s = acc; m = bm;
         } else
-        for (int c0 = sub; c0 < nblk; c0 += 64) {  // 8 independent (max, sum) pairs in flight per lane
+        for (int c0 = sub; c0 < nblk; c0 += 64) {  // larger grids: 8 independent (max, sum) pairs in flight per lane
           float mm[8], ss[8];
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
@@ -601,109 +507,22 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
   int cur = 0, iters = 0;
   bool converged = false;
   double err = 1.0, prev_check_err = -1.0;
-  const bool single = fact && p.atomic_cols != 0;
-  if (single) {
-    // ---- single-barrier iteration: column partials reduced by fixed-point atomics, ONE grid barrier per sweep ----
-    // acc[3][n1p] (zeroed by the launcher) lives in the part_s workspace; sweep s adds into acc[s % 3], after the
-    // barrier every thread reads the totals of ITS columns and forms v_new itself (no combine phase, no second
-    // barrier); buffer (s + 2) % 3 -- last read one barrier ago -- is zeroed by slices for the sweep after next.
-    // v is kept per CTA in the part_m workspace row b (each thread re-reads only what it wrote).
-    unsigned long long* acc = reinterpret_cast<unsigned long long*>(p.part_s);
-    float* vmine = part_m + (int64_t)b * n1p;
-    // v used by the sweep that produced the totals being absorbed lives in vmine (this thread's own columns)
-#pragma unroll
-    for (int k = 0; k < KG; ++k)
-      if (gvalid[k]) *reinterpret_cast<float4*>(vmine + tcol + kV2Consumers * 4 * k) = make_float4(0.f, 0.f, 0.f, 0.f);
-    float vref_cur = 0.f;
-    const int cpc = ((n1 + nblk - 1) / nblk + 3) & ~3;
-    sweep(false, true, nullptr, nullptr, 0.f, acc, nullptr);
-    grid_sync();
-    for (int it = 0;; ++it) {
-      const unsigned long long* tot = acc + (size_t)(it % 3) * n1p;
-      {  // zero this CTA's slice of the buffer of sweep it + 2
-        unsigned long long* z = acc + (size_t)((it + 2) % 3) * n1p;
-        for (int j = b * cpc + tid; j < min(n1, (b + 1) * cpc); j += kV2Threads) z[j] = 0ull;
-      }
-      // totals t_j = 2^(v_j - v_new_j) of this thread's columns (and of column 0, the common reference)
-      float4 vnew[KG];
-      double e2 = 0.0;
-      const float t0 = (float)((double)__ldcg(tot) * 2.3283064365386963e-10);
-      const float vref_new = vref_cur - lg2_abs(t0);
-#pragma unroll
-      for (int k = 0; k < KG; ++k) {
-        float4 vcur_k = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (gvalid[k]) vcur_k = __ldcg(reinterpret_cast<const float4*>(vmine + tcol + kV2Consumers * 4 * k));
-        vnew[k] = vcur_k;
-        if (gvalid[k]) {
-          const ulonglong2 a = __ldcg(reinterpret_cast<const ulonglong2*>(tot + tcol + kV2Consumers * 4 * k));
-          const ulonglong2 c = __ldcg(reinterpret_cast<const ulonglong2*>(tot + tcol + kV2Consumers * 4 * k + 2));
-          const double td[4] = {(double)a.x * 2.3283064365386963e-10, (double)a.y * 2.3283064365386963e-10,
-                                (double)c.x * 2.3283064365386963e-10, (double)c.y * 2.3283064365386963e-10};
-          vnew[k] = make_float4(vcur_k.x - lg2_abs((float)td[0]), vcur_k.y - lg2_abs((float)td[1]),
-                                vcur_k.z - lg2_abs((float)td[2]), vcur_k.w - lg2_abs((float)td[3]));
-#pragma unroll
-          for (int q = 0; q < 4; ++q) e2 += (td[q] - 1.0) * (td[q] - 1.0);
-        }
-      }
-      // stopping rule of iteration it - 1 (POT: every check_every iterations, column marginal of (u, v) in L2 norm):
-      // expm1(v_prev - v_new) = t - 1.  Every CTA evaluates it on the same numbers in the same order.
-      if (it >= 1 && (((it - 1) % p.check_every) == 0 || (p.dbg_flags & 2))) {
-        e2 = warp_sum(e2);
-        if (lane == 0) red[warp] = e2;
-        __syncthreads();
-        double t = 0.0;
-        for (int w = 0; w < kV2Warps; ++w) t += red[w];
-        __syncthreads();
-        err = sqrt(t) / (double)n1;
-        if (((it - 1) % p.check_every) == 0) {
-          if (err < p.stop_thr) { converged = true; break; }
-          if (p.stall_tol > 0.0 && prev_check_err >= 0.0 && err > (1.0 - p.stall_tol) * prev_check_err &&
-              err * sqrt((double)n1) < 1e-5) { converged = true; break; }
-          prev_check_err = err;
-        }
-      }
-      if (it == p.max_iters) break;  // (only reached when the last iteration ran its column phase for a check)
-#pragma unroll
-      for (int k = 0; k < KG; ++k)
-        if (gvalid[k]) *reinterpret_cast<float4*>(vmine + tcol + kV2Consumers * 4 * k) = vnew[k];
-      vref_cur = vref_new;
-      const bool last = (it == p.max_iters - 1);
-      const bool check = (it % p.check_every) == 0;
-      const bool do_col = !last || check;
-      sweep(true, do_col, nullptr, vnew, vref_cur, do_col ? acc + (size_t)((it + 1) % 3) * n1p : nullptr, vmine);
-      iters = it + 1;
-      if (!do_col) break;
-      grid_sync();
-    }
-    // outputs: v of the last sweep (parked in vmine by this very thread), u written by the sweep
-    if (b == 0) {
-#pragma unroll
-      for (int k = 0; k < KG; ++k)
-        if (gvalid[k]) {
-          const int j = tcol + kV2Consumers * 4 * k;
-          const float4 vv = __ldcg(reinterpret_cast<const float4*>(vmine + j));
-          p.log_v[j] = (double)vv.x * kLn2d; p.log_v[j + 1] = (double)vv.y * kLn2d;
-          p.log_v[j + 2] = (double)vv.z * kLn2d; p.log_v[j + 3] = (double)vv.w * kLn2d;
-        }
-    }
-  } else {
-  sweep(false, true, nullptr, nullptr, 0.f, nullptr, nullptr);
-  grid_sync();
+  sweep(false, true, nullptr);
+  grid.sync();
   combine(nullptr, v_work[0], false, nullptr);
-  grid_sync();
+  grid.sync();
 
   for (int it = 0; it < p.max_iters; ++it) {
     const bool last = (it == p.max_iters - 1);
     const bool check = (it % p.check_every) == 0;
     const bool do_col = !last || check;
-    sweep(true, do_col, v_work[cur], nullptr, 0.f, nullptr, nullptr);
+    sweep(true, do_col, v_work[cur]);
     iters = it + 1;
     if (!do_col) break;
-    grid_sync();
+    grid.sync();
     if (b == 0 && tid == 0) p.err_ring[(it + 2) & 3] = 0.0;
-    const bool want_err = check || (p.dbg_flags & 2);
-    combine(v_work[cur], v_work[cur ^ 1], want_err, want_err ? &p.err_ring[it & 3] : nullptr);
-    grid_sync();
+    combine(v_work[cur], v_work[cur ^ 1], check, check ? &p.err_ring[it & 3] : nullptr);
+    grid.sync();
     if (check) {
       err = sqrt(__ldcg(&p.err_ring[it & 3]));
       if (err < p.stop_thr) { converged = true; break; }
@@ -714,7 +533,6 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
     if (last) break;
     cur ^= 1;
   }
-  }  // two-barrier path
 
   // ---- drain speculative prefetches so no bulk copy is in flight when the CTA exits ----
   if (tid == 0) {
@@ -724,9 +542,8 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
     }
   }
 
-  if (!single)
-    for (int j = b * kV2Threads + tid; j < n1; j += nblk * kV2Threads)
-      p.log_v[j] = (double)__ldcg(v_work[cur] + j) * kLn2d;
+  for (int j = b * kV2Threads + tid; j < n1; j += nblk * kV2Threads)
+    p.log_v[j] = (double)__ldcg(v_work[cur] + j) * kLn2d;
   if (b == 0 && tid == 0) {
     int flags = 0;
     if (!converged) flags |= CFM_FLAG_NOT_CONVERGED;
@@ -734,7 +551,7 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
     p.status[0] = flags;
     p.status[1] = iters;
     p.status[2] = 0;
-    p.status[3] = fact ? (single ? 4 : 3) : 2;  // kernel variant: 4 = factored + single barrier, 3 = factored, 2 = log-domain
+    p.status[3] = fact ? 3 : 2;  // kernel variant: 3 = factored, 2 = log-domain
     *p.err_out = err;
   }
 }
@@ -742,11 +559,9 @@ __global__ void __launch_bounds__(NT, 512 / NT) sinkhorn_v2_kernel(const SkParam
 template <int NT, int KG, int R>
 static int v2_launch_t(SkParams& p, cudaStream_t s) {
   auto kern = sinkhorn_v2_kernel<NT, KG, R>;
-  constexpr int kPerSm = 512 / NT;
   const size_t stage_bytes = (size_t)R * p.n1p * 4;
-  const size_t fixed = (size_t)2 * R * (NT / 32) * sizeof(float2) + 8 * sizeof(uint64_t) + 128 +
-                       (KG > 4 ? (size_t)p.n1p * 4 : 0);
-  const size_t budget = (kPerSm == 1 ? 220 : 108) * 1024;
+  const size_t fixed = (size_t)2 * R * (NT / 32) * sizeof(float2) + 8 * sizeof(uint64_t) + 128;
+  const size_t budget = 220 * 1024;
   if (budget < fixed + 2 * stage_bytes) return 1;
   int S = (int)((budget - fixed) / stage_bytes);
   if (S > 8) S = 8;
@@ -755,13 +570,9 @@ static int v2_launch_t(SkParams& p, cudaStream_t s) {
   int per_sm = 0;
   CFM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, NT, smem));
   if (per_sm < 1) return 1;
-  if (per_sm > kPerSm) per_sm = kPerSm;
-  int grid = sm_count() * per_sm;
+  int grid = sm_count();
   if (grid > p.n0) grid = p.n0;
   void* args[] = {(void*)&p, (void*)&S};
-  CFM_CUDA_OK(cudaMemsetAsync(p.err_ring + 4, 0, 16, s));  // grid-barrier counter
-  if (p.atomic_cols)  // the three fixed-point column accumulators of the single-barrier mode
-    CFM_CUDA_OK(cudaMemsetAsync(p.part_s, 0, (size_t)3 * p.n1p * sizeof(unsigned long long), s));
   CFM_CUDA_OK(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(NT), args, smem, s));
   note_launches(1);
   return CFM_OK;
@@ -782,40 +593,8 @@ int sinkhorn_v2_launch(SkParams& p, cudaStream_t s) {
   static float l2frac = -2.f;
   if (l2frac < -1.f) { const char* e = getenv("CFM_SK_L2"); l2frac = e ? (float)atof(e) : -1.f; }
   p.l2_resident_frac = !streams ? 0.f : l2frac >= 0.f ? l2frac : fminf(1.f, kSkResidentShare * (float)l2 / (float)m_bytes);
-  static int dbg = -1;  // CFM_SK_DBG: A/B switches (bit0: 4-wide combine loop, bit2: 8-wide loop, bit1: marginal error every iteration)
-  // default (0): all partials of a lane loaded in one round trip
-  if (dbg < 0) { const char* e = getenv("CFM_SK_DBG"); dbg = e ? atoi(e) : 0; }
-  p.dbg_flags = dbg;
-  static int pf = -1;  // CFM_SK_PF: chunks (of R rows) per CTA prefetched into L2 at the end of every sweep
-  // the prefetched rows displace the evict_last resident part of the slabs from L2, so the default is off
-  if (pf < 0) { const char* e = getenv("CFM_SK_PF"); pf = e ? atoi(e) : 0; }
-  p.prefetch_chunks = streams ? pf : 0;  // pointless when M lives in L2 anyway
-  static int atom = -1;  // CFM_SK_ATOMIC: 1 = single-barrier iteration (fixed-point atomic column sums), 0 = two barriers + combine
-  // default off: two barriers + the sliced combine instead of 1.2 M 64-bit L2 atomics per iteration at N = 8192
-  if (atom < 0) { const char* e = getenv("CFM_SK_ATOMIC"); atom = e ? atoi(e) : 0; }
-  p.atomic_cols = atom;
-  static long persist = -2;  // CFM_SK_PERSIST_MB: raise cudaLimitPersistingL2CacheSize before the first solve (experiment)
-  if (persist == -2) {
-    const char* e = getenv("CFM_SK_PERSIST_MB");
-    persist = e ? atol(e) : -1;
-    if (persist >= 0) cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)persist << 20);
-  }
-  static int cfg = -1;  // CFM_SK_CONFIG: 0 heuristic (default), 1 force 512-thread CTAs, 2 force 256-thread CTAs
-  if (cfg < 0) { const char* e = getenv("CFM_SK_CONFIG"); cfg = e ? atoi(e) : 0; }
-  const int ng = p.n1p / 4;
-  // default: one 512-thread CTA per SM
-#ifdef CFM_SK_BUILD_256  // experiment only (measured slower): two 256-thread CTAs per SM
-  if (cfg == 2) {
-    const int kg = (ng + 255) / 256;
-    int rc = 1;
-    if (kg <= 1) rc = v2_launch_t<256, 1, 8>(p, s);
-    else if (kg <= 2) rc = v2_launch_t<256, 2, 4>(p, s);
-    else if (kg <= 4) rc = v2_launch_t<256, 4, 2>(p, s);
-    else rc = v2_launch_t<256, 8, 1>(p, s);
-    if (rc != 1) return rc;
-  }
-#endif
-  const int kg = (ng + 511) / 512;
+  // one 512-thread CTA per SM
+  const int kg = (p.n1p / 4 + 511) / 512;
   if (kg <= 1) return v2_launch_t<512, 1, 8>(p, s);
   if (kg <= 2) return v2_launch_t<512, 2, 4>(p, s);
   return v2_launch_t<512, 4, 2>(p, s);

@@ -1,11 +1,10 @@
 // Cost matrix  M = torch.cdist(x0, x1) ** 2   (reference: torchcfm/optimal_transport.py:84)
 //
 // HBM layout: x0 (n0,d), x1 (n1,d) fp32 row-major; M (n0,n1) fp32 row-major, row stride ldm.
-// Two code paths behind cfm_sqdist_f32:
+// Two code paths behind cfm_sqdist_f32 (algo 0 = auto picks one of them; 2, a retired 3xTF32 path, is refused):
 //   algo 1  SIMT fp32 FMA GEMM (gemm_simt.cuh)      -- any shape / alignment
-//   algo 2  wgmma 3xTF32 GEMM (sqdist_tc.cu)        -- d % 4 == 0, 16B-aligned rows
-//   algo 3  wgmma fp16x3 GEMM (sqdist_h3.cu)        -- same shapes, twice the tensor rate (auto mode's choice)
-// Both share the row-norm pre-pass and the epilogue
+//   algo 3  wgmma fp16x3 GEMM (sqdist_h3.cu)        -- d % 4 == 0, 16B-aligned rows
+// Both apply the epilogue
 //   M_ij = (sqrt(max(|x0_i|^2 + |x1_j|^2 - 2 <x0_i, x1_j>, 0)))^2
 // which follows ATen's _euclidean_dist (clamp_min(0).sqrt()) and the reference's `** 2`.
 #include "gemm_simt.cuh"
@@ -65,13 +64,11 @@ struct SqDistEpilogue {
   }
 };
 
-// implemented in sqdist_tc.cu
-int sqdist_tc_supported(int n0, int n1, int d, const float* x0, const float* x1, const float* M,
-                        int64_t ldm);
-size_t sqdist_tc_workspace_bytes(int n0, int n1, int d);
-int sqdist_tc_launch(const float* x0, const float* x1, float* M, int n0, int n1, int d,
-                     int64_t ldm, int squared, float* cost_max, const float* nx, const float* ny,
-                     void* ws, size_t ws_bytes, cudaStream_t s);
+// shapes the tensor-core path takes: whole 16-byte units per row, 16-byte aligned operands
+static bool tc_supported(int d, const float* x0, const float* x1, const float* M, int64_t ldm) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(x0) | reinterpret_cast<uintptr_t>(x1) | reinterpret_cast<uintptr_t>(M);
+  return (d % 4 == 0) && (a % 16 == 0) && (ldm % 4 == 0);
+}
 
 // implemented in sqdist_h3.cu (fp16x3 scheme; the pre-pass also writes the row norms)
 size_t sqdist_h3_workspace_bytes(int n0, int n1, int d);
@@ -88,8 +85,7 @@ using namespace cfm;
 
 extern "C" size_t cfm_sqdist_workspace_bytes(int n0, int n1, int d, int algo) {
   size_t b = norms_bytes(n0, n1);
-  if (algo == 2) b += sqdist_tc_workspace_bytes(n0, n1, d);
-  else if (algo != 1) b += sqdist_h3_workspace_bytes(n0, n1, d);  // auto / 3
+  if (algo != 1) b += sqdist_h3_workspace_bytes(n0, n1, d);  // auto / 3
   return b;
 }
 
@@ -100,13 +96,11 @@ extern "C" int cfm_sqdist_f32(const float* x0, const float* x1, float* M, int n0
   CFM_REQUIRE(x0 && x1 && M, "cfm_sqdist_f32: null pointer");
   CFM_REQUIRE(n0 > 0 && n1 > 0 && d > 0 && ldm >= n1, "cfm_sqdist_f32: bad shape n0=%d n1=%d d=%d ldm=%lld",
               n0, n1, d, (long long)ldm);
-  CFM_REQUIRE(algo >= 0 && algo <= 3, "cfm_sqdist_f32: unknown algo %d", algo);
-  const bool tc_ok = sqdist_tc_supported(n0, n1, d, x0, x1, M, ldm) != 0;
-  if (algo >= 2) CFM_REQUIRE(tc_ok, "cfm_sqdist_f32: tensor-core paths need d %% 4 == 0, 16B-aligned x0/x1/M and ldm %% 4 == 0");
+  CFM_REQUIRE(algo == 0 || algo == 1 || algo == 3, "cfm_sqdist_f32: unknown algo %d", algo);
+  const bool tc_ok = tc_supported(d, x0, x1, M, ldm);
+  if (algo == 3) CFM_REQUIRE(tc_ok, "cfm_sqdist_f32: tensor-core path needs d %% 4 == 0, 16B-aligned x0/x1/M and ldm %% 4 == 0");
   const bool use_h3 = (algo == 3) || (algo == 0 && tc_ok && (int64_t)n0 * n1 >= 256 * 256 && d >= 32);
-  const bool use_tc = (algo == 2);
-  const size_t need = norms_bytes(n0, n1) + (use_tc ? sqdist_tc_workspace_bytes(n0, n1, d) : 0) +
-                      (use_h3 ? sqdist_h3_workspace_bytes(n0, n1, d) : 0);
+  const size_t need = norms_bytes(n0, n1) + (use_h3 ? sqdist_h3_workspace_bytes(n0, n1, d) : 0);
   CFM_REQUIRE(workspace && workspace_bytes >= need, "cfm_sqdist_f32: workspace too small (%zu < %zu)",
               workspace_bytes, need);
   float* nx = reinterpret_cast<float*>(workspace);
@@ -120,10 +114,6 @@ extern "C" int cfm_sqdist_f32(const float* x0, const float* x1, float* M, int n0
   row_sqnorm_kernel<<<(n0 + 7) / 8, 256, 0, s>>>(x0, n0, d, nx); ::cfm::note_launches(1);
   row_sqnorm_kernel<<<(n1 + 7) / 8, 256, 0, s>>>(x1, n1, d, ny); ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
-  if (use_tc) {
-    return sqdist_tc_launch(x0, x1, M, n0, n1, d, ldm, squared, cost_max, nx, ny, tcws,
-                            workspace_bytes - norms_bytes(n0, n1), s);
-  }
   SqDistEpilogue epi{nx, ny, M, ldm, cost_max, squared, 0.f};
   CFM_CUDA_OK(launch_gemm_nt_simt(x0, (int64_t)d, x1, (int64_t)d, n0, n1, d, epi, s));
   return CFM_OK;

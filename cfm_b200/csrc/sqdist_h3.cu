@@ -5,10 +5,82 @@
 // row scale s_r that puts max|x_r| * s_r in [2^13, 2^14) (exact; fp16 overflows at 65504 and the data range
 // is the caller's), and the (hi, lo) fp16 split of the scaled row.  The GEMM epilogue undoes the scales --
 // dot_ij = (acc0 + acc1 2^-11) / (s_i t_j), again exact powers of two -- and applies
-// |x0_i|^2 + |x1_j|^2 - 2 dot, clamp, sqrt, square, running max exactly like the other two paths.
+// |x0_i|^2 + |x1_j|^2 - 2 dot, clamp, sqrt, square, running max exactly like the SIMT path (sqdist.cu).
+#include <mutex>
+
 #include "gemm_h3.cuh"
 
 namespace cfm {
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
+                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                  CUtensorMapFloatOOBfill);
+
+static EncodeTiledFn encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  }
+  return fn;
+}
+
+// ---- TMA descriptor cache ---------------------------------------------------------------------------
+// A CUtensorMap is a pure function of (base pointer, shape, strides, box, element type); a training loop
+// hands the same buffers to the GEMMs every step, so the encode call is made once per distinct key and the
+// 128-byte descriptor is replayed from a small direct-mapped table afterwards (the only library state
+// besides the error string; guarded by a mutex, safe from several host threads).
+namespace {
+struct MapKey {
+  const void* base; int rows, d, box_rows, elem; int64_t ld;
+  bool operator==(const MapKey& o) const {
+    return base == o.base && rows == o.rows && d == o.d && box_rows == o.box_rows && elem == o.elem && ld == o.ld;
+  }
+};
+struct MapSlot { MapKey key; CUtensorMap map; bool used; };
+constexpr int kMapSlots = 256;
+MapSlot g_maps[kMapSlots];
+std::mutex g_map_mu;
+inline unsigned map_hash(const MapKey& k) {
+  uint64_t h = reinterpret_cast<uintptr_t>(k.base) * 0x9E3779B97F4A7C15ull;
+  h ^= ((uint64_t)k.rows << 32) ^ (uint64_t)k.d ^ ((uint64_t)k.box_rows << 20) ^ ((uint64_t)k.elem << 12) ^ ((uint64_t)k.ld << 40);
+  h *= 0xC2B2AE3D27D4EB4Full;
+  return (unsigned)(h >> 40) % kMapSlots;
+}
+}  // namespace
+
+static int make_map_cached(CUtensorMap* m, const void* base, int rows, int d, int64_t ld, int box_rows, int elem) {
+  const MapKey key{base, rows, d, box_rows, elem, ld};
+  const unsigned slot = map_hash(key);
+  {
+    std::lock_guard<std::mutex> g(g_map_mu);
+    if (g_maps[slot].used && g_maps[slot].key == key) { *m = g_maps[slot].map; return CFM_OK; }
+  }
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) { set_error("cuTensorMapEncodeTiled not available from the driver"); return CFM_ERR_CUDA; }
+  cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * (cuuint64_t)elem};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / elem), (cuuint32_t)box_rows};  // 128-byte swizzle atom wide
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(m, elem == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
+                  const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed (%d) rows=%d d=%d ld=%lld elem=%d", (int)r, rows, d, (long long)ld, elem);
+    return CFM_ERR_CUDA;
+  }
+  std::lock_guard<std::mutex> g(g_map_mu);
+  g_maps[slot].key = key; g_maps[slot].map = *m; g_maps[slot].used = true;
+  return CFM_OK;
+}
+
+int tc_make_map_f16(CUtensorMap* m, const __half* base, int rows, int d, int64_t ld, int box_rows) {
+  return make_map_cached(m, base, rows, d, ld, box_rows, 2);
+}
 
 // one warp per row; d % 4 == 0, x 16-byte aligned, ldo % 8 == 0.  `uniform_absmax` (nullable, device): scale every
 // row by the power of two derived from THIS value instead of the row's own maximum (the MLP weights: one scale per

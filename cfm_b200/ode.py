@@ -158,7 +158,7 @@ class NeuralODE(torch.nn.Module):
         for stage in range(1, 7) if not (P["rkfused"] or (split and P["overlap"])) else ():
             out = xs if stage < 6 else xnew
             if split:
-                # the stage input goes straight to the MLP as its TF32 operand pair; only stage 6
+                # the stage input goes straight to the MLP as its fp16x3 (hi, lo) operand pair; only stage 6
                 # (= xnew, needed by the error norm and the commit) is also kept in fp32
                 _ffi.check(L.cfm_rk_stage_input(stp, _ffi.ptr(x), _ffi.ptr(k), _ffi.ptr(out if stage == 6 else None),
                                                 _ffi.ptr(P["xs_hi"]), _ffi.ptr(P["xs_lo"]), _ffi.ptr(P["t_stage"]),

@@ -102,7 +102,7 @@ class OTPlanSampler:
         'fp32-generic' forces the fp32 arithmetic onto the generic kernel: cross-checks).
     stall_tol : stop once an fp32 fixed point is reached (see include/cfm_b200.h); 0 disables.
     cost_algo : 0 auto (fp16x3 tensor-core path for aligned shapes; SIMT for exact OT), 1 SIMT fp32,
-        2 wgmma 3xTF32 (round-1 path, kept for A/B), 3 wgmma fp16x3.
+        3 wgmma fp16x3.
     """
 
     def __init__(
@@ -140,6 +140,8 @@ class OTPlanSampler:
             raise ValueError(f"Unknown precision: {precision}")
         self.precision = precision
         self.stall_tol = float(stall_tol)
+        if cost_algo not in (0, 1, 3):
+            raise ValueError(f"Unknown cost_algo: {cost_algo}")
         self.cost_algo = int(cost_algo)
         self._last_info = {}
         self._pending = collections.deque()  # deferred status words of warn=False calls (event, pinned, coupling)

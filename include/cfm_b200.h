@@ -52,18 +52,14 @@ long long cfm_launch_count(void);
  * un-squared distance otherwise (wasserstein power=1, :297).
  * cost_max (nullable, 1 float): receives max_ij M_ij (the M.max() of :86); must be
  * zeroed by the caller... it is zeroed by this call.
- * algo: 0 auto, 1 SIMT fp32 FMA, 2 wgmma 3xTF32 (error-compensated, fp32-grade), 3 wgmma fp16x3
- * (x = hi + lo 2^-11 in fp16, three fp16 wgmma MMAs into two accumulators; same fp32-grade accuracy at twice
- * the tensor rate and half the operand bytes; what auto picks for aligned shapes).
+ * algo: 0 auto, 1 SIMT fp32 FMA, 3 wgmma fp16x3 (x = hi + lo 2^-11 in fp16, three fp16 wgmma MMAs into two
+ * accumulators: fp32-grade accuracy; what auto picks for aligned shapes).  Any other value, 2 included (a
+ * retired 3xTF32 path), fails with "unknown algo".
  */
 size_t cfm_sqdist_workspace_bytes(int n0, int n1, int d, int algo);
 int cfm_sqdist_f32(const float* x0, const float* x1, float* M, int n0, int n1, int d,
                    int64_t ldm, int squared, float* cost_max, int algo, void* workspace,
                    size_t workspace_bytes, void* stream);
-
-/* profiling aid: per-CTA %globaltimer checkpoints of the following tensor-core GEMM launches are written
- * to buf (device, >= 8 * sm_count uint64); NULL switches it off.  Not used on the product path. */
-int cfm_tc_debug_buffer(unsigned long long* buf);
 
 /* ---- (a4) entropic plan: log-domain Sinkhorn on uniform marginals ---------------
  * replaces pot.sinkhorn(a, b, M, reg) as bound at optimal_transport.py:51 and called

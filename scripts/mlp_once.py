@@ -1,4 +1,4 @@
-"""One fused MLP forward at BASELINE config 3's shape (input of the ncu capture of mlp_fused_h3_kernel)."""
+"""One fused MLP forward at BASELINE config 3's shape (a short run for a profiler capture of mlp_fused_h3_kernel)."""
 import sys
 import torch
 sys.path.insert(0, '.')

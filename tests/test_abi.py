@@ -40,6 +40,19 @@ def test_library_holds_sm90a_code_only(lib_built):
     assert arches == {"90a"}, arches
 
 
+def test_sqdist_refuses_algo_2(lib_built):
+    """cfm_sqdist_f32 checks algo before any CUDA call; 2 (the retired 3xTF32 path) is an argument error.  The
+    pointers are dummies that are never dereferenced, and the workspace is declared too small as well, so no build
+    of the library gets as far as a launch."""
+    from cfm_b200 import _ffi
+    lib = _ffi.load_library(lib_built)
+    buf = ctypes.create_string_buffer(256)
+    p = ctypes.addressof(buf)
+    rc = lib.cfm_sqdist_f32(p, p, p, 4, 4, 4, 4, 1, None, 2, p, 0, None)
+    assert rc == -1  # CFM_ERR_ARG
+    assert b"unknown algo" in lib.cfm_last_error()
+
+
 def test_rk_state_struct_layout_matches_header():
     from cfm_b200 import _ffi
     assert ctypes.sizeof(_ffi.RkState) == 72

@@ -36,6 +36,14 @@ def test_ctor_contract():
     assert cfm_b200.ExactOptimalTransportConditionalFlowMatcher().ot_sampler.method == "exact"
 
 
+def test_cost_algo_2_is_refused():
+    """Cost-matrix algo 2 (the 3xTF32 path fp16x3 replaced) is gone: the sampler refuses it when constructed."""
+    with pytest.raises(ValueError, match="Unknown cost_algo: 2"):
+        OTPlanSampler("exact", cost_algo=2)
+    for algo in (0, 1, 3):
+        assert OTPlanSampler("sinkhorn", cost_algo=algo).cost_algo == algo
+
+
 def test_signatures_match_reference_source():
     """Compare public signatures with the reference *source* (parsed by tests/golden/make_golden_glue.py)."""
     import json
