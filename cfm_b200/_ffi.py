@@ -61,18 +61,11 @@ SIGNATURES = {
     "cfm_mlp_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "cfm_mlp_forward_f32": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _f, _i, _p, _i, _p, _sz, _p]),
     "cfm_mlp_tc_supported": (_i, [_i, _i, _i, _i]),
-    "cfm_mlp_forward_split_f32": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _f, _i, _p, _p, _sz, _p]),
     "cfm_mlp_forward_split_gated_f32": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _f, _i, _p, _p, _p, _sz, _p]),
-    "cfm_mlp_rkstage_supported": (_i, [_i, _i, _i, _i]),
-    "cfm_mlp_forward_rkstage_f32": (_i, [_p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _p, _sz, _p]),
     "cfm_rk_stage_input": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i64, _i, _p]),
-    "cfm_rk_stage_partial": (_i, [_p, _p, _p, _p, _p, _p, _i64, _i, _p]),
-    "cfm_rk_stage_finish": (_i, [_p, _p, _p, _p, _p, _p, _p, _i64, _i, _p]),
     "cfm_rk_error_norm": (_i, [_p, _p, _p, _p, _p, _i64, _p]),
     "cfm_rk_control": (_i, [_p, _p, _i64, _p]),
     "cfm_rk_commit": (_i, [_p, _p, _p, _p, _p, _i64, _p]),
-    "cfm_rk_init_a": (_i, [_p, _p, _p, _p, _p, _p, _i64, _p]),
-    "cfm_rk_init_b": (_i, [_p, _p, _p, _p, _p, _p, _i64, _p]),
     "cfm_rk_init_sums": (_i, [_p, _p, _p, _p, _p, _i64, _i, _p]),
     "cfm_rk_init_probe": (_i, [_p, _p, _p, _p, _p, _p, _i64, _i64, _p]),
     "cfm_rk_init_finish": (_i, [_p, _p, _p, _i64, _p]),

@@ -13,7 +13,6 @@
 // FMA, the numerics of the reference's cuBLAS sgemm with TF32 off).
 #include "gemm_simt.cuh"
 #include "mlp_common.cuh"
-#include "rk_tableau.h"
 
 namespace cfm {
 
@@ -122,7 +121,7 @@ extern "C" int cfm_mlp_forward_f32(const void* prepared, const float* x, int bat
   const char* B = reinterpret_cast<const char*>(prepared);
   if (use_tc)
     return mlp_tc_forward(h, prepared, x, nullptr, nullptr, batch, t_dev, t_host, act, y, workspace,
-                          workspace_bytes, nullptr, nullptr, s);
+                          workspace_bytes, nullptr, s);
   auto P = [&](int64_t off) { return reinterpret_cast<const float*>(B + off); };
   float* hA = reinterpret_cast<float*>(workspace);
   float* hB = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + align_up((size_t)batch * w * 4, 256));
@@ -141,52 +140,16 @@ extern "C" int cfm_mlp_tc_supported(int batch, int dim, int w, int out_dim) {
   return mlp_tc_supported(batch, dim, w, out_dim);
 }
 
-extern "C" int cfm_mlp_forward_split_f32(const void* prepared, const void* x_hi, const void* x_lo, int batch,
-                                         int dim, int w, int out_dim, int time_varying, const float* t_dev,
-                                         float t_host, int act, float* y, void* workspace,
-                                         size_t workspace_bytes, void* stream) {
-  return cfm_mlp_forward_split_gated_f32(prepared, x_hi, x_lo, batch, dim, w, out_dim, time_varying, t_dev, t_host,
-                                         act, y, nullptr, workspace, workspace_bytes, stream);
-}
-
 extern "C" int cfm_mlp_forward_split_gated_f32(const void* prepared, const void* x_hi, const void* x_lo, int batch,
                                                int dim, int w, int out_dim, int time_varying, const float* t_dev,
                                                float t_host, int act, float* y, const int32_t* skip_if_nonzero,
                                                void* workspace, size_t workspace_bytes, void* stream) {
-  CFM_REQUIRE(prepared && x_hi && x_lo && y && workspace, "cfm_mlp_forward_split_f32: null pointer");
-  CFM_REQUIRE(act == CFM_ACT_SELU || act == CFM_ACT_SILU, "cfm_mlp_forward_split_f32: unknown activation %d", act);
+  CFM_REQUIRE(prepared && x_hi && x_lo && y && workspace, "cfm_mlp_forward_split_gated_f32: null pointer");
+  CFM_REQUIRE(act == CFM_ACT_SELU || act == CFM_ACT_SILU,
+              "cfm_mlp_forward_split_gated_f32: unknown activation %d", act);
   CFM_REQUIRE(mlp_tc_supported(batch, dim, w, out_dim) != 0,
-              "cfm_mlp_forward_split_f32: shape not supported by the tensor-core path");
+              "cfm_mlp_forward_split_gated_f32: shape not supported by the tensor-core path");
   const MlpBlobHeader h = mlp_layout(dim, w, out_dim, time_varying ? 1 : 0);
   return mlp_tc_forward(h, prepared, nullptr, x_hi, x_lo, batch, t_dev, t_host, act, y, workspace,
-                        workspace_bytes, skip_if_nonzero, nullptr, (cudaStream_t)stream);
-}
-
-extern "C" int cfm_mlp_rkstage_supported(int batch, int dim, int w, int out_dim) {
-  return mlp_tc_rkstage_supported(batch, dim, w, out_dim);
-}
-
-extern "C" int cfm_mlp_forward_rkstage_f32(const void* prepared, const cfm_rk_state* st, const float* x, float* k,
-                                           int stage, float* xnew, float* err_partial, int batch, int dim, int w,
-                                           int out_dim, int act, void* workspace, size_t workspace_bytes,
-                                           void* stream) {
-  static const float kc[7] = CFM_RK_C_INIT;
-  static const float ka[7][6] = CFM_RK_A_INIT;
-  static const float ke[7] = CFM_RK_E_INIT;
-  CFM_REQUIRE(prepared && st && x && k && workspace, "cfm_mlp_forward_rkstage_f32: null pointer");
-  CFM_REQUIRE(stage >= 1 && stage <= 6, "cfm_mlp_forward_rkstage_f32: stage must be in 1..6 (got %d)", stage);
-  CFM_REQUIRE(err_partial == nullptr || stage == 6, "cfm_mlp_forward_rkstage_f32: err_partial belongs to stage 6");
-  CFM_REQUIRE(act == CFM_ACT_SELU || act == CFM_ACT_SILU, "cfm_mlp_forward_rkstage_f32: unknown activation %d", act);
-  CFM_REQUIRE(mlp_tc_rkstage_supported(batch, dim, w, out_dim) != 0,
-              "cfm_mlp_forward_rkstage_f32: shape not supported (see cfm_mlp_rkstage_supported)");
-  const MlpBlobHeader h = mlp_layout(dim, w, out_dim, 1);
-  MlpRkStage rk;
-  rk.x = x; rk.k = k; rk.numel = (int64_t)batch * dim;
-  rk.h_dev = &st->dt; rk.t0_dev = &st->t;
-  for (int j = 0; j < 6; ++j) { rk.coef[j] = j < stage ? ka[stage][j] : 0.f; rk.ecoef[j] = ke[j]; }
-  rk.c = kc[stage];
-  rk.xnew = xnew; rk.err = err_partial;
-  float* y = k + (int64_t)stage * rk.numel;  // k_{stage+1}
-  return mlp_tc_forward(h, prepared, nullptr, nullptr, nullptr, batch, nullptr, 0.f, act, y, workspace,
-                        workspace_bytes, &st->done, &rk, (cudaStream_t)stream);
+                        workspace_bytes, skip_if_nonzero, (cudaStream_t)stream);
 }

@@ -14,22 +14,9 @@ size_t mlp_tc_blob_bytes(int dim, int w, int out_dim);  // mlp_h3.cu
 int mlp_tc_prepare(const MlpBlobHeader& h, void* blob, cudaStream_t s);
 int mlp_tc_supported(int batch, int dim, int w, int out_dim);
 size_t mlp_tc_workspace_bytes(int batch, int dim, int w, int out_dim);
-// A dopri5 stage input formed inside the fused kernel (mlp_h3.cu, RK mode):
-//   v = x + sum_j (h * coef[j]) k_j,  k_j = k + j * numel,  evaluated at  t0 + c * h  (h, t0: device scalars)
-struct MlpRkStage {
-  const float* x;
-  const float* k;
-  int64_t numel;
-  const float* h_dev;
-  const float* t0_dev;
-  float coef[6], ecoef[6], c;
-  float* xnew;  // nullable: fp32 copy of v
-  float* err;   // nullable: sum_j ecoef[j] k_j
-};
-int mlp_tc_rkstage_supported(int batch, int dim, int w, int out_dim);
 int mlp_tc_forward(const MlpBlobHeader& h, const void* blob, const float* x, const void* x_hi,
                    const void* x_lo, int batch, const float* t_dev, float t_host, int act, float* y, void* ws,
-                   size_t ws_bytes, const int32_t* skip, const MlpRkStage* rk, cudaStream_t s);
+                   size_t ws_bytes, const int32_t* skip, cudaStream_t s);
 
 static inline MlpBlobHeader mlp_layout(int dim, int w, int out_dim, int tv) {
   MlpBlobHeader h;

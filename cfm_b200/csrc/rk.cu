@@ -153,80 +153,6 @@ rk_stage_input_kernel(const cfm_rk_state* __restrict__ st, const float* __restri
   }
 }
 
-// Split form of the stage input, for overlap with the vector-field evaluation: the part of
-//   xs_s = x + dt * sum_{j<s} a[s][j] k_j
-// that does not need the newest derivative k_s (j = s-1), P_s = x + dt * sum_{j<s-1} a[s][j] k_j, only needs what is
-// known one evaluation earlier, so it runs on a side stream WHILE the MLP computes k_s; afterwards a light kernel
-// adds the last term and writes the operand pair.  Same fp32 operations in the same order as the one-piece kernel,
-// hence bit-identical stage inputs.  Stage 6 also carries the embedded error estimate's partial sum.
-__global__ void rk_stage_partial_kernel(const cfm_rk_state* __restrict__ st, const float* __restrict__ x,
-                                        const float* __restrict__ k, float* __restrict__ partial,
-                                        float* __restrict__ err_partial, float* __restrict__ t_stage, int64_t numel,
-                                        int stage) {
-  if (st->done) return;
-  const float dt = st->dt;
-  if (blockIdx.x == 0 && threadIdx.x == 0 && t_stage) *t_stage = fmaf(kC[stage], dt, st->t);
-  float a[6];
-#pragma unroll
-  for (int j = 0; j < 6; ++j) a[j] = dt * kA[stage][j];
-  const int64_t n4 = numel >> 2;  // (launcher requires numel % 4 == 0)
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 v = reinterpret_cast<const float4*>(x)[i];
-    float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {
-      if (j < stage - 1 && kA[stage][j] != 0.f) {
-        const float4 kk = reinterpret_cast<const float4*>(k + (int64_t)j * numel)[i];
-        v.x = fmaf(a[j], kk.x, v.x); v.y = fmaf(a[j], kk.y, v.y);
-        v.z = fmaf(a[j], kk.z, v.z); v.w = fmaf(a[j], kk.w, v.w);
-        if (err_partial) {
-          e.x = fmaf(kE[j], kk.x, e.x); e.y = fmaf(kE[j], kk.y, e.y);
-          e.z = fmaf(kE[j], kk.z, e.z); e.w = fmaf(kE[j], kk.w, e.w);
-        }
-      }
-    }
-    reinterpret_cast<float4*>(partial)[i] = v;
-    if (err_partial) reinterpret_cast<float4*>(err_partial)[i] = e;
-  }
-}
-
-// xs_s = P_s + dt * a[s][s-1] * k_s  -> fp32 (stage 6: xnew) and / or the fp16x3 operand pair; stage 6 also finishes
-// the error partial in place: err_partial += e_6 * k_6
-__global__ void rk_stage_finish_kernel(const cfm_rk_state* __restrict__ st, const float* __restrict__ partial,
-                                       const float* __restrict__ k, float* __restrict__ out,
-                                       __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                                       float* __restrict__ err_partial, int64_t numel, int stage) {
-  if (st->done) return;
-  const float a = st->dt * kA[stage][stage - 1];
-  const float ke = kE[stage - 1];
-  const float* kl = k + (int64_t)(stage - 1) * numel;
-  const int64_t n4 = numel >> 2;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 v = reinterpret_cast<const float4*>(partial)[i];
-    const float4 kk = reinterpret_cast<const float4*>(kl)[i];
-    v.x = fmaf(a, kk.x, v.x); v.y = fmaf(a, kk.y, v.y); v.z = fmaf(a, kk.z, v.z); v.w = fmaf(a, kk.w, v.w);
-    if (err_partial) {
-      float4 e = reinterpret_cast<const float4*>(err_partial)[i];
-      e.x = fmaf(ke, kk.x, e.x); e.y = fmaf(ke, kk.y, e.y); e.z = fmaf(ke, kk.z, e.z); e.w = fmaf(ke, kk.w, e.w);
-      reinterpret_cast<float4*>(err_partial)[i] = e;
-    }
-    if (out) reinterpret_cast<float4*>(out)[i] = v;
-    if (out_hi) {
-      __half h[4], l[4];
-      rk_split_h3(v.x, h[0], l[0]); rk_split_h3(v.y, h[1], l[1]);
-      rk_split_h3(v.z, h[2], l[2]); rk_split_h3(v.w, h[3], l[3]);
-      reinterpret_cast<uint2*>(out_hi)[i] = make_uint2(
-          (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
-          (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16));
-      reinterpret_cast<uint2*>(out_lo)[i] = make_uint2(
-          (uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16),
-          (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16));
-    }
-  }
-}
-
 // err_acc += sum( (dt * sum_j e_j k_j / (atol + rtol * max(|x|, |xnew|)))^2 )
 __global__ void rk_error_norm_kernel(cfm_rk_state* st, const float* __restrict__ x,
                                      const float* __restrict__ xnew, const float* __restrict__ k,
@@ -439,32 +365,6 @@ extern "C" int cfm_rk_stage_input(const cfm_rk_state* st, const float* x, const 
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
 }
-extern "C" int cfm_rk_stage_partial(const cfm_rk_state* st, const float* x, const float* k, float* partial,
-                                    float* err_partial, float* t_stage, int64_t numel, int stage, void* stream) {
-  RK_CHECK(st && x && k && partial && numel > 0 && (numel & 3) == 0 && stage >= 2 && stage <= 6);
-  RK_CHECK(err_partial == nullptr || stage == 6);
-  RK_CHECK(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(partial) |
-             reinterpret_cast<uintptr_t>(err_partial)) & 15) == 0);
-  rk_stage_partial_kernel<<<ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, k, partial, err_partial, t_stage,
-                                                                           numel, stage); ::cfm::note_launches(1);
-  CFM_CUDA_OK(cudaGetLastError());
-  return CFM_OK;
-}
-extern "C" int cfm_rk_stage_finish(const cfm_rk_state* st, const float* partial, const float* k, float* out,
-                                   void* out_hi, void* out_lo, float* err_partial, int64_t numel, int stage,
-                                   void* stream) {
-  RK_CHECK(st && partial && k && (out || out_hi) && numel > 0 && (numel & 3) == 0 && stage >= 2 && stage <= 6);
-  RK_CHECK((out_hi == nullptr) == (out_lo == nullptr));
-  RK_CHECK(err_partial == nullptr || stage == 6);
-  RK_CHECK(((reinterpret_cast<uintptr_t>(partial) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(out) |
-             reinterpret_cast<uintptr_t>(out_hi) | reinterpret_cast<uintptr_t>(out_lo) |
-             reinterpret_cast<uintptr_t>(err_partial)) & 15) == 0);
-  rk_stage_finish_kernel<<<ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(
-      st, partial, k, out, reinterpret_cast<__half*>(out_hi), reinterpret_cast<__half*>(out_lo), err_partial, numel,
-      stage); ::cfm::note_launches(1);
-  CFM_CUDA_OK(cudaGetLastError());
-  return CFM_OK;
-}
 extern "C" int cfm_rk_error_norm(cfm_rk_state* st, const float* x, const float* xnew, const float* k,
                                  const float* err_partial, int64_t numel, void* stream) {
   RK_CHECK(st && x && xnew && k && numel > 0);
@@ -485,20 +385,9 @@ extern "C" int cfm_rk_commit(const cfm_rk_state* st, float* x, const float* xnew
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
 }
-extern "C" int cfm_rk_init_a(cfm_rk_state* st, const float* x, const float* f0, float* x_probe,
-                             float* t_stage, double* scratch, int64_t numel, void* stream) {
-  int rc = cfm_rk_init_sums(st, x, f0, nullptr, scratch, numel, 0, stream);
-  if (rc != CFM_OK) return rc;
-  return cfm_rk_init_probe(st, x, f0, x_probe, t_stage, scratch, numel, numel, stream);
-}
-extern "C" int cfm_rk_init_b(cfm_rk_state* st, const float* x, const float* f0, const float* f1,
-                             const float* t_span, double* scratch, int64_t numel, void* stream) {
-  int rc = cfm_rk_init_sums(st, x, f0, f1, scratch, numel, 1, stream);
-  if (rc != CFM_OK) return rc;
-  return cfm_rk_init_finish(st, t_span, scratch, numel, stream);
-}
-// the same four steps one by one, so that a sharded (lock-step) driver can all-reduce the partial sums in
-// `scratch` between them and pass the GLOBAL element count to the steps that turn sums into norms
+// The Hairer initial step in four calls (sums phase 0, probe, sums phase 1, finish), so that a sharded (lock-step)
+// driver can all-reduce the partial sums in `scratch` between them and pass the GLOBAL element count to the steps
+// that turn sums into norms
 extern "C" int cfm_rk_init_sums(const cfm_rk_state* st, const float* x, const float* f0, const float* f1,
                                 double* scratch, int64_t numel, int phase, void* stream) {
   RK_CHECK(st && x && f0 && scratch && numel > 0 && (phase == 0 || (phase == 1 && f1)));

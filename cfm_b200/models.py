@@ -145,29 +145,6 @@ class MLP(torch.nn.Module):
         return out
 
 
-    def rkstage_path(self, batch):
-        """True when a dopri5 stage evaluation of this field runs as ONE launch (stage input formed inside the fused
-        MLP kernel, cfm_mlp_forward_rkstage_f32)."""
-        if self.mlp_algo == 1 or not self.time_varying:
-            return False
-        return bool(_ffi.lib().cfm_mlp_rkstage_supported(batch, self.net[0].in_features - 1, self.w, self.out_dim))
-
-    def vector_field_rkstage(self, state, x, k, stage, xnew=None, err_partial=None):
-        """k[stage] = f(t + c dt, x + dt sum_j a[stage][j] k[j]) with t, dt read from the device-resident controller
-        ``state`` (cfm_rk_state as a uint8 CUDA tensor); ``k``: (7, B, D) fp32."""
-        L = _ffi.lib()
-        dev = x.device
-        dim = self.net[0].in_features - 1
-        B = x.shape[0]
-        blob = self._prepared(True, dev)
-        ws = _ffi.workspace(L.cfm_mlp_workspace_bytes(B, dim, self.w, self.out_dim, 2), dev)
-        _ffi.check(L.cfm_mlp_forward_rkstage_f32(
-            _ffi.ptr(blob), _ffi.ptr(state), _ffi.ptr(x), _ffi.ptr(k), int(stage), _ffi.ptr(xnew), _ffi.ptr(err_partial),
-            B, dim, self.w, self.out_dim, self.act, _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)),
-            "cfm_mlp_forward_rkstage_f32")
-        return k[stage]
-
-
 class torch_wrapper(torch.nn.Module):
     """Wraps model to torchdyn compatible format (reference torchcfm/utils.py:44-52)."""
 

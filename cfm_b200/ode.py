@@ -58,15 +58,6 @@ class NeuralODE(torch.nn.Module):
         # per step attempt, three more for the initial step) are all-reduced so that every rank takes exactly
         # the step sequence a single process would take on the full batch.
         self.lockstep = None
-        # True: compute the bulk of every stage input on a side stream during the previous MLP evaluation
-        # (cfm_rk_stage_partial / _finish).  Bit-identical; off by default: the partial kernels compete with the MLP's
-        # operand feed for L2 / HBM bandwidth and the finish kernels add launches, so the default is the one-piece
-        # stage input on one stream.
-        self.overlap_stages = False
-        # True (default): a stage evaluation is ONE launch -- the stage input x + dt sum a_sj k_j is formed inside the
-        # fused MLP kernel as its layer-1 operand producer (cfm_mlp_forward_rkstage_f32; bit-identical to the separate
-        # stage-input kernel, which remains the path of other widths and of fuse_stage_input = False)
-        self.fuse_stage_input = False
         self._plans = {}
 
     @torch.no_grad()
@@ -150,12 +141,7 @@ class NeuralODE(torch.nn.Module):
         sp = _ffi.stream_ptr(P["dev"])
         stp, x, xnew, xs, k, numel = P["stp"], P["x"], P["xnew"], P["xs"], P["k"], P["numel"]
         split = P["xs_hi"] is not None
-        if P["rkfused"]:
-            for stage in range(1, 7):  # stage input + evaluation in one launch; stage 6 leaves xnew and the error partial
-                mlp.vector_field_rkstage(P["st"], x, k, stage, xnew if stage == 6 else None, xs if stage == 6 else None)
-        elif split and P["overlap"]:
-            self._enqueue_stages_overlapped(mlp, P)
-        for stage in range(1, 7) if not (P["rkfused"] or (split and P["overlap"])) else ():
+        for stage in range(1, 7):
             out = xs if stage < 6 else xnew
             if split:
                 # the stage input goes straight to the MLP as its fp16x3 (hi, lo) operand pair; only stage 6
@@ -170,60 +156,16 @@ class NeuralODE(torch.nn.Module):
                                                 _ffi.ptr(P["t_stage"]), None, numel, stage, sp), "cfm_rk_stage_input")
                 mlp.vector_field(P["t_stage"], out, out=k[stage])
         _ffi.check(L.cfm_rk_error_norm(stp, _ffi.ptr(x), _ffi.ptr(xnew), _ffi.ptr(k),
-                                       _ffi.ptr(xs if (split or P["rkfused"]) else None), numel, sp), "cfm_rk_error_norm")
+                                       _ffi.ptr(xs if split else None), numel, sp), "cfm_rk_error_norm")
         if P["group"] is not None:  # lock-step: the error norm is over the rows of ALL ranks
             P["dist"].all_reduce(P["err_acc"], group=P["group"])
         _ffi.check(L.cfm_rk_control(stp, _ffi.ptr(P["t_span"]), P["numel_global"], sp), "cfm_rk_control")
         _ffi.check(L.cfm_rk_commit(stp, _ffi.ptr(x), _ffi.ptr(xnew), _ffi.ptr(k), _ffi.ptr(P["traj"]),
                                    numel, sp), "cfm_rk_commit")
 
-    def _enqueue_stages_overlapped(self, mlp, P):
-        """The six stage evaluations of a step with the bulk of every stage input computed on a side stream WHILE the
-        MLP evaluates the previous stage: the input of stage s is  P_s + dt a[s][s-1] k_s  where
-        P_s = x + dt sum_{j<s-1} a[s][j] k_j  does not need the newest derivative (cfm_rk_stage_partial, side stream,
-        forked as soon as k_{s-1} exists) and the last term is added by a light kernel after the MLP
-        (cfm_rk_stage_finish).  Bit-identical to the one-piece form; works eagerly and under graph capture
-        (fork / join through events).  Stage times: slot s % 2 of P["t_slots"]."""
-        L = _ffi.lib()
-        dev = P["dev"]
-        main = torch.cuda.current_stream(dev)
-        side = P["side"]
-        stp, x, xnew, xs, k, numel = P["stp"], P["x"], P["xnew"], P["xs"], P["k"], P["numel"]
-        hi, lo, tsl, pb = P["xs_hi"], P["xs_lo"], P["t_slots"], P["pbuf"]
-        msp = _ffi.stream_ptr(dev)
-
-        def fork_partial(stage):  # P_stage on the side stream; returns the event that marks it done
-            ev = torch.cuda.Event()
-            ev.record(main)
-            side.wait_event(ev)
-            with torch.cuda.stream(side):
-                _ffi.check(L.cfm_rk_stage_partial(stp, _ffi.ptr(x), _ffi.ptr(k), _ffi.ptr(pb[stage % 2]),
-                                                  _ffi.ptr(xs if stage == 6 else None), _ffi.ptr(tsl[stage % 2]),
-                                                  numel, stage, _ffi.stream_ptr(dev)), "cfm_rk_stage_partial")
-                done = torch.cuda.Event()
-                done.record(side)
-            return done
-
-        # stage 1 needs k1 only: one piece
-        _ffi.check(L.cfm_rk_stage_input(stp, _ffi.ptr(x), _ffi.ptr(k), None, _ffi.ptr(hi), _ffi.ptr(lo),
-                                        _ffi.ptr(tsl[1]), None, numel, 1, msp), "cfm_rk_stage_input")
-        pending = fork_partial(2)  # P_2 = x + dt a20 k1: also needs k1 only
-        for e in range(1, 7):      # evaluation e: input = stage input e (in hi / lo), output k[e] = k_{e+1}
-            mlp.vector_field_split(tsl[e % 2], hi, lo, k[e], skip_flag=P["done_flag"])
-            if e == 6:
-                break
-            nxt = fork_partial(e + 2) if e + 2 <= 6 else None  # needs k_1 .. k_{e+1}: all there now
-            main.wait_event(pending)
-            s = e + 1
-            _ffi.check(L.cfm_rk_stage_finish(stp, _ffi.ptr(pb[s % 2]), _ffi.ptr(k), _ffi.ptr(xnew if s == 6 else None),
-                                             _ffi.ptr(hi), _ffi.ptr(lo), _ffi.ptr(xs if s == 6 else None), numel, s,
-                                             msp), "cfm_rk_stage_finish")
-            pending = nxt
-
     def _plan(self, mlp, B, D, n_span, dev):
         """Persistent buffers (+ the captured step graph) for one problem shape and weight version."""
-        key = (id(mlp), B, D, n_span, str(dev), mlp._weights_key(), mlp.mlp_algo, mlp.act, self.lockstep is not None,
-               self.overlap_stages, self.fuse_stage_input)
+        key = (id(mlp), B, D, n_span, str(dev), mlp._weights_key(), mlp.mlp_algo, mlp.act, self.lockstep is not None)
         P = self._plans.get(key)
         if P is not None:
             return P
@@ -241,8 +183,7 @@ class NeuralODE(torch.nn.Module):
              "pinned": torch.empty(ctypes_sizeof_state(), dtype=torch.uint8, pin_memory=True),
              "pinned_init": torch.empty(ctypes_sizeof_state(), dtype=torch.uint8, pin_memory=True),
              "t0": torch.zeros(1, dtype=torch.float32, device=dev), "ts_host": None, "init_graph": None,
-             "xs_hi": None, "xs_lo": None, "graph": None, "group": None, "dist": None, "numel_global": B * D,
-             "overlap": False, "rkfused": False}
+             "xs_hi": None, "xs_lo": None, "graph": None, "group": None, "dist": None, "numel_global": B * D}
         off = _ffi.RkState.err_acc.offset  # the float64 accumulator inside the device state struct
         P["err_acc"] = st[off:off + 8].view(torch.float64)
         off = _ffi.RkState.done.offset  # int32: non-zero once t has reached t_end
@@ -251,12 +192,6 @@ class NeuralODE(torch.nn.Module):
             # stage inputs go to the MLP as its fp16x3 tensor-core operand pair (hi, lo), written by the RK kernel
             P["xs_hi"] = torch.empty((B, D), dtype=torch.float16, device=dev)
             P["xs_lo"] = torch.empty((B, D), dtype=torch.float16, device=dev)
-            P["rkfused"] = bool(self.fuse_stage_input and not self.overlap_stages and mlp.rkstage_path(B))
-            if self.overlap_stages and (B * D) % 4 == 0:
-                P["overlap"] = True
-                P["side"] = torch.cuda.Stream(dev)
-                P["pbuf"] = [torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(2)]
-                P["t_slots"] = [torch.zeros(1, dtype=torch.float32, device=dev) for _ in range(2)]
         self._plans[key] = P
         return P
 

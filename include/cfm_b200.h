@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define CFM_ABI_VERSION 1
+#define CFM_ABI_VERSION 2
 
 #define CFM_OK 0
 #define CFM_ERR_ARG (-1)   /* bad argument (shape, alignment, null pointer, workspace too small) */
@@ -212,15 +212,11 @@ int cfm_mlp_forward_f32(const void* prepared, const float* x, int batch, int dim
  * (fp16 arrays of B*dim elements: x_hi = fp16(x), x_lo = fp16((x - x_hi) * 2048), as written by
  * cfm_rk_stage_input); tensor-core paths only: ONE fused persistent launch for 256-wide hidden layers
  * (activations stay in shared memory), per-layer GEMM launches otherwise.  cfm_mlp_tc_supported() != 0
- * tells whether a shape runs on them. */
+ * tells whether a shape runs on them.  Device-side gate: when *skip_if_nonzero != 0 (nullable) the fused kernel
+ * returns at once.  The dopri5 driver passes &state->done, so that steps enqueued speculatively after the
+ * integration has finished cost a launch, not a forward (the per-layer path ignores the gate: its result is simply
+ * unused). */
 int cfm_mlp_tc_supported(int batch, int dim, int w, int out_dim);
-int cfm_mlp_forward_split_f32(const void* prepared, const void* x_hi, const void* x_lo, int batch,
-                              int dim, int w, int out_dim, int time_varying, const float* t_dev,
-                              float t_host, int act, float* y, void* workspace,
-                              size_t workspace_bytes, void* stream);
-/* The same with a device-side gate: when *skip_if_nonzero != 0 (nullable) the fused kernel returns at once.  The
- * dopri5 driver passes &state->done, so that steps enqueued speculatively after the integration has finished cost a
- * launch, not a forward (the per-layer path ignores the gate: its result is simply unused). */
 int cfm_mlp_forward_split_gated_f32(const void* prepared, const void* x_hi, const void* x_lo, int batch,
                                     int dim, int w, int out_dim, int time_varying, const float* t_dev,
                                     float t_host, int act, float* y, const int32_t* skip_if_nonzero,
@@ -252,37 +248,13 @@ typedef struct cfm_rk_state {
 /* stage in 1..5: out = x + dt*sum_j a[stage][j]*k_j (input of stage+1's evaluation);
  * stage 6: the same with the 5th-order weights, i.e. out = xnew (and the FSAL input).
  * out (nullable) receives the fp32 value; out_hi/out_lo (nullable pair, fp16 arrays of numel elements)
- * receive its fp16x3 operand split, the form cfm_mlp_forward_split_f32 consumes.  *t_stage (device
+ * receive its fp16x3 operand split, the form cfm_mlp_forward_split_gated_f32 consumes.  *t_stage (device
  * float, nullable) = t + c[stage]*dt.  err_partial (nullable, stage 6 only, numel floats): receives
  * sum_{j<=6} e_j k_j, the first six terms of the embedded error estimate -- stage 6 reads k1..k6 anyway, so
  * cfm_rk_error_norm can then read four arrays instead of eight. */
 int cfm_rk_stage_input(const cfm_rk_state* st, const float* x, const float* k, float* out,
                        void* out_hi, void* out_lo, float* t_stage, float* err_partial, int64_t numel,
                        int stage, void* stream);
-/* The stage input in two pieces, so that the bulk of it overlaps the vector-field evaluation that precedes it
- * (stage in 2..6, numel % 4 == 0):  cfm_rk_stage_partial writes  partial = x + dt*sum_{j<stage-1} a[stage][j]*k_j
- * -- everything that does not need the newest derivative k_stage -- and *t_stage; it can run on a side stream
- * while the MLP computes k_stage.  cfm_rk_stage_finish then forms  partial + dt*a[stage][stage-1]*k_stage  and
- * writes it like cfm_rk_stage_input does.  Same fp32 operations in the same order: bit-identical stage inputs.
- * err_partial (nullable, stage 6): partial writes sum_{j<5} e_j k_j, finish adds e_6 k_6 in place. */
-int cfm_rk_stage_partial(const cfm_rk_state* st, const float* x, const float* k, float* partial,
-                         float* err_partial, float* t_stage, int64_t numel, int stage, void* stream);
-int cfm_rk_stage_finish(const cfm_rk_state* st, const float* partial, const float* k, float* out, void* out_hi,
-                        void* out_lo, float* err_partial, int64_t numel, int stage, void* stream);
-/* One dopri5 stage EVALUATION in one launch (256-wide vector-field MLPs with out_dim == dim; cfm_mlp_rkstage_supported()
- * != 0 tells whether a shape qualifies):  k_{stage+1} = f(t + c[stage] dt, x + dt sum_{j<stage} a[stage][j] k_j).
- * The stage input is formed INSIDE the fused MLP kernel, as the layer-1 operand producer (the same fp32 operations in
- * the same order as cfm_rk_stage_input, hence bit-identical results), so it neither makes a separate pass over
- * x, k_1..k_stage nor round-trips through HBM as an fp16 pair.  k: the 7 contiguous derivative arrays (k_{stage+1} =
- * k + stage * batch * dim is written); xnew (nullable) receives the fp32 stage input (stage 6: the candidate state),
- * err_partial (nullable, stage 6 only) the first six terms of the embedded error estimate.  Returns at once when
- * st->done != 0.  `prepared` must have been built with time_varying = 1.  Replaces, per NFE, the reference's
- * torch.cat([x, t]) + 4 nn.Linear + 3 SELU (torchcfm/utils.py:51-52, models/models.py:10-21) and torchdyn's stage
- * combination. */
-int cfm_mlp_rkstage_supported(int batch, int dim, int w, int out_dim);
-int cfm_mlp_forward_rkstage_f32(const void* prepared, const cfm_rk_state* st, const float* x, float* k, int stage,
-                                float* xnew, float* err_partial, int batch, int dim, int w, int out_dim, int act,
-                                void* workspace, size_t workspace_bytes, void* stream);
 /* st->err_acc += sum((dt*sum_j e_j k_j / (atol + rtol*max(|x|,|xnew|)))^2); with err_partial (see above) the
  * sum over j is err_partial + e_7 k_7 */
 int cfm_rk_error_norm(cfm_rk_state* st, const float* x, const float* xnew, const float* k,
@@ -292,17 +264,13 @@ int cfm_rk_control(cfm_rk_state* st, const float* t_span, int64_t numel, void* s
 /* if the step was accepted: x <- xnew, k1 <- k7 (FSAL), traj[save_slot] <- xnew */
 int cfm_rk_commit(const cfm_rk_state* st, float* x, const float* xnew, float* k, float* traj,
                   int64_t numel, void* stream);
-/* Hairer initial step (torchdyn init_step) around the f(t0+h0, x+h0*f0) evaluation:
- * init_a writes x_probe and *t_stage; init_b finishes dt and clips it.  scratch: 4 doubles. */
-int cfm_rk_init_a(cfm_rk_state* st, const float* x, const float* f0, float* x_probe,
-                  float* t_stage, double* scratch, int64_t numel, void* stream);
-int cfm_rk_init_b(cfm_rk_state* st, const float* x, const float* f0, const float* f1,
-                  const float* t_span, double* scratch, int64_t numel, void* stream);
-/* The same initial-step computation in its four stages, for row-sharded (lock-step) integration across
- * ranks (SURVEY section 8e): cfm_rk_init_sums accumulates this shard's partial sums into scratch
- * (phase 0: zeroes scratch, then sum (x/scale)^2 and sum (f0/scale)^2; phase 1: sum ((f1-f0)/scale)^2);
- * the driver all-reduces scratch over the ranks; probe / finish then take the GLOBAL element count.
- * cfm_rk_control's numel is likewise the global count when st->err_acc has been all-reduced. */
+/* Hairer initial step (torchdyn init_step) around the f(t0+h0, x+h0*f0) evaluation, in four calls so that
+ * row-sharded (lock-step) integration across ranks (SURVEY section 8e) can all-reduce between them:
+ * cfm_rk_init_sums accumulates this shard's partial sums into scratch (4 doubles; phase 0: zeroes scratch, then
+ * sum (x/scale)^2 and sum (f0/scale)^2; phase 1: sum ((f1-f0)/scale)^2); the driver all-reduces scratch over the
+ * ranks; cfm_rk_init_probe (writes x_probe and *t_stage) and cfm_rk_init_finish (finishes dt and clips it) then
+ * take the GLOBAL element count.  cfm_rk_control's numel is likewise the global count when st->err_acc has been
+ * all-reduced. */
 int cfm_rk_init_sums(const cfm_rk_state* st, const float* x, const float* f0, const float* f1,
                      double* scratch, int64_t numel, int phase, void* stream);
 int cfm_rk_init_probe(cfm_rk_state* st, const float* x, const float* f0, float* x_probe, float* t_stage,

@@ -22,11 +22,14 @@ def test_header_and_binding_agree():
     assert sorted(_ffi.SIGNATURES) == declared
 
 
-def test_library_loads_and_exports_every_symbol(lib_built):
+def test_library_loads_exports_every_symbol_and_reports_the_header_abi_version(lib_built):
     from cfm_b200 import _ffi
     assert os.path.exists(lib_built)
     lib = _ffi.load_library(lib_built)  # binds every name in SIGNATURES or raises
-    assert lib.cfm_abi_version() == 1
+    header = open(os.path.join(ROOT, "include", "cfm_b200.h")).read()
+    declared_version = int(re.search(r"#define\s+CFM_ABI_VERSION\s+(\d+)", header).group(1))
+    assert declared_version == 2  # 2: the stage-variant and unused dopri5 / MLP entry points were removed
+    assert lib.cfm_abi_version() == declared_version
     raw = ctypes.CDLL(lib_built)
     for name in _declared_symbols():
         assert hasattr(raw, name), name

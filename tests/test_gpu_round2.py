@@ -326,13 +326,13 @@ def test_dopri5_config3_full_batch_one_launch_per_nfe():
     assert node.stats["nfe"] == st["nfe"] == 20 and node.stats["accepted"] == st["accepted"]
     assert (traj[-1].cpu() - ref[-1]).abs().max() <= 1e-4 * ref.abs().max()
     # initial step: 2 x (fp32 -> fp16x3 split + fused MLP) + 2 reductions + probe + finish = 8 launches;
-    # per step: stage-1 input + 5 x (partial on the side stream + finish) + 6 x ONE fused MLP launch + error norm +
-    # control + commit = 20 (15 with the one-piece stage inputs).  Four launches per forward would need 38.
+    # per step: 6 x (stage input + ONE fused MLP launch) + error norm + control + commit = 15.  Four launches per
+    # forward would need 33.
     steps = node.stats["accepted"] + node.stats["rejected"]
-    assert launches <= 8 + (steps + 1) * 20, (launches, steps)
+    assert launches <= 8 + (steps + 1) * 15, (launches, steps)
 
 
-# ------------------------------------------------------------------------- dopri5 driver, split stage inputs
+# ------------------------------------------------------------------------- dopri5 driver, stage inputs
 def _rk_state(dt=0.0625, t=0.25):
     st = _ffi.RkState()
     st.t, st.dt, st.t_end, st.atol, st.rtol = t, dt, 1.0, 1e-4, 1e-4
@@ -340,61 +340,43 @@ def _rk_state(dt=0.0625, t=0.25):
     return torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(DEV)
 
 
-@pytest.mark.parametrize("stage", [2, 3, 4, 5, 6])
-def test_rk_stage_partial_plus_finish_is_bit_identical_to_the_one_piece_kernel(stage):
-    """cfm_rk_stage_partial (everything but the newest derivative; runs on a side stream during the MLP) followed by
-    cfm_rk_stage_finish performs the same fp32 operations in the same order as cfm_rk_stage_input."""
+@pytest.mark.parametrize("stage", [1, 2, 3, 4, 5, 6])
+def test_rk_stage_input_operand_pair_and_stage6_outputs(stage):
+    """cfm_rk_stage_input: the (hi, lo) operand pair is the fp16x3 split of the fp32 stage input; at stage 6 the fp32
+    output (xnew) and the error partial match float64 arithmetic on the same inputs."""
     L = _ffi.lib()
     B, D = 513, 64
     numel = B * D
+    dt = 0.0625
     g = torch.Generator().manual_seed(stage)
-    x = torch.randn(B, D, generator=g).to(DEV)
-    k = torch.randn(7, B, D, generator=g).to(DEV)
-    st = _rk_state()
+    x = torch.randn(B, D, generator=g)
+    k = torch.randn(7, B, D, generator=g)
+    st = _rk_state(dt=dt)
     sp = _ffi.stream_ptr(torch.device(DEV))
-    f32 = lambda: torch.zeros(B, D, dtype=torch.float32, device=DEV)  # noqa: E731
-    f16 = lambda: torch.zeros(B, D, dtype=torch.float16, device=DEV)  # noqa: E731
-    out_a, hi_a, lo_a, e_a, t_a = f32(), f16(), f16(), f32(), torch.zeros(1, device=DEV)
-    _ffi.check(L.cfm_rk_stage_input(_ffi.ptr(st), _ffi.ptr(x), _ffi.ptr(k), _ffi.ptr(out_a), _ffi.ptr(hi_a), _ffi.ptr(lo_a),
-                                    _ffi.ptr(t_a), _ffi.ptr(e_a) if stage == 6 else None, numel, stage, sp), "stage_input")
-    part, out_b, hi_b, lo_b, e_b, t_b = f32(), f32(), f16(), f16(), f32(), torch.zeros(1, device=DEV)
-    _ffi.check(L.cfm_rk_stage_partial(_ffi.ptr(st), _ffi.ptr(x), _ffi.ptr(k), _ffi.ptr(part),
-                                      _ffi.ptr(e_b) if stage == 6 else None, _ffi.ptr(t_b), numel, stage, sp), "partial")
-    _ffi.check(L.cfm_rk_stage_finish(_ffi.ptr(st), _ffi.ptr(part), _ffi.ptr(k), _ffi.ptr(out_b), _ffi.ptr(hi_b), _ffi.ptr(lo_b),
-                                     _ffi.ptr(e_b) if stage == 6 else None, numel, stage, sp), "finish")
-    assert torch.equal(out_a, out_b) and torch.equal(t_a, t_b)
-    assert torch.equal(hi_a.view(torch.int16), hi_b.view(torch.int16)) and torch.equal(lo_a.view(torch.int16), lo_b.view(torch.int16))
+    out = torch.zeros(B, D, dtype=torch.float32, device=DEV)
+    hi, lo = (torch.zeros(B, D, dtype=torch.float16, device=DEV) for _ in range(2))
+    errp, t_s = torch.zeros(B, D, dtype=torch.float32, device=DEV), torch.zeros(1, device=DEV)
+    xd, kd = x.to(DEV), k.to(DEV)
+    _ffi.check(L.cfm_rk_stage_input(_ffi.ptr(st), _ffi.ptr(xd), _ffi.ptr(kd), _ffi.ptr(out), _ffi.ptr(hi), _ffi.ptr(lo),
+                                    _ffi.ptr(t_s), _ffi.ptr(errp) if stage == 6 else None, numel, stage, sp),
+               "stage_input")
+    rec = hi.float() + lo.float() / 2048.0
+    assert (rec - out).abs().max().item() <= 2.0 ** -21 * out.abs().max().item()
     if stage == 6:
-        assert torch.equal(e_a, e_b)
-    # and the operand pair is the fp16x3 split of the fp32 stage input
-    rec = hi_b.float() + lo_b.float() / 2048.0
-    assert (rec - out_b).abs().max().item() <= 2.0 ** -21 * out_b.abs().max().item()
-
-
-def test_dopri5_overlapped_stage_inputs_equal_the_serial_driver():
-    """Trajectories with the stage inputs split across two streams (graph and eager) are bit-identical to the serial
-    one-stream driver: same kernels' arithmetic, only the schedule differs."""
-    torch.manual_seed(0)
-    m = cfm_b200.MLP(dim=64, w=256, time_varying=True).to(DEV)
-    x = torch.randn(1500, 64, generator=torch.Generator().manual_seed(1)).to(DEV)
-    span = torch.linspace(0, 1, 4)
-    outs = []
-    for overlap, graph in ((False, True), (True, True), (True, False)):
-        node = cfm_b200.NeuralODE(cfm_b200.torch_wrapper(m), solver="dopri5", atol=1e-5, rtol=1e-5)
-        node.overlap_stages, node.use_cuda_graph = overlap, graph
-        node.trajectory(x, span)
-        outs.append((node.trajectory(x, span).clone(), dict(node.stats)))
-    for o, s in outs[1:]:
-        assert torch.equal(o, outs[0][0])
-        assert (s["nfe"], s["accepted"], s["rejected"]) == (outs[0][1]["nfe"], outs[0][1]["accepted"], outs[0][1]["rejected"])
+        A6 = [35 / 384, 0.0, 500 / 1113, 125 / 192, -2187 / 6784, 11 / 84]
+        E = [35 / 384 - 1951 / 21600, 0.0, 500 / 1113 - 22642 / 50085, 125 / 192 - 451 / 720,
+             -2187 / 6784 + 12231 / 42400, 11 / 84 - 649 / 6300]
+        xs = x.double() + dt * sum(a * k[j].double() for j, a in enumerate(A6))
+        ep = sum(e * k[j].double() for j, e in enumerate(E))
+        assert (out.cpu().double() - xs).abs().max() <= 4e-6 * xs.abs().max()
+        assert (errp.cpu().double() - ep).abs().max() <= 4e-6 * max(1.0, ep.abs().max().item())
 
 
 @pytest.mark.parametrize("B,dim,act", [(1500, 64, "selu"), (1000, 784, "selu"), (300, 200, "silu")])
-def test_dopri5_stage_input_formed_inside_the_fused_mlp_equals_the_separate_kernel(B, dim, act):
-    """cfm_mlp_forward_rkstage_f32 (stage input formed by the fused MLP kernel's layer-1 operand producer, one launch per
-    NFE) against the two-launch form (cfm_rk_stage_input + cfm_mlp_forward_split_gated_f32): the same fp32 operations
-    in the same order, so trajectories, step counts and the controller's error ratios are bit-identical -- on ragged
-    slabs (B % 128 != 0), a ragged last K chunk (784 = 12 x 64 + 16; 200 = 3 x 64 + 8) and both activations."""
+def test_dopri5_graph_and_eager_drivers_give_identical_trajectories(B, dim, act):
+    """The captured CUDA-graph step and the eagerly enqueued step run the same kernels on the same buffers, so
+    trajectories, step counts and the controller's error ratios are bit-identical -- on ragged slabs (B % 128 != 0),
+    a ragged last K chunk (784 = 12 x 64 + 16; 200 = 3 x 64 + 8) and both activations."""
     torch.manual_seed(3)
     m = cfm_b200.MLP(dim=dim, w=256, time_varying=True).to(DEV)
     if act == "silu":
@@ -402,55 +384,16 @@ def test_dopri5_stage_input_formed_inside_the_fused_mlp_equals_the_separate_kern
     x = torch.randn(B, dim, generator=torch.Generator().manual_seed(4)).to(DEV)
     span = torch.linspace(0, 1, 3)
     outs = []
-    for fuse, graph in ((False, True), (True, True), (True, False)):
+    for graph in (True, False):
         node = cfm_b200.NeuralODE(cfm_b200.torch_wrapper(m), solver="dopri5", atol=1e-5, rtol=1e-5)
-        node.fuse_stage_input, node.use_cuda_graph = fuse, graph
+        node.use_cuda_graph = graph
         node.trajectory(x, span)
         outs.append((node.trajectory(x, span).clone(), dict(node.stats)))
-        P = next(iter(node._plans.values()))
-        assert P["rkfused"] == fuse
-    for o, s in outs[1:]:
-        assert torch.equal(o, outs[0][0])
-        assert (s["nfe"], s["accepted"], s["rejected"], s["last_ratio"]) == \
-            (outs[0][1]["nfe"], outs[0][1]["accepted"], outs[0][1]["rejected"], outs[0][1]["last_ratio"])
-
-
-def test_rkstage_single_evaluation_against_the_float64_oracle():
-    """One stage evaluation through the one-launch form, checked directly: k_{s+1}, xnew and the error partial against
-    float64 arithmetic on the same inputs (1e-5 of max|y| for the field, fp32 rounding for the combinations)."""
-    from oracle import vector_field as vf
-    torch.manual_seed(5)
-    B, D = 777, 784
-    m = cfm_b200.MLP(dim=D, w=256, time_varying=True)
-    sd = {k_: v_.clone() for k_, v_ in m.state_dict().items()}
-
-    def f64(t, z):  # utils.py:51-52 + models.py:20-21 in float64
-        return vf.mlp_forward_from_state(sd, torch.cat([z.double(), torch.full((z.shape[0], 1), t, dtype=torch.float64)], 1))
-    m = m.to(DEV)
-    g = torch.Generator().manual_seed(6)
-    x = torch.randn(B, D, generator=g)
-    k = torch.randn(7, B, D, generator=g)
-    st = _ffi.RkState()
-    st.t, st.dt, st.t_end, st.atol, st.rtol = 0.25, 0.125, 1.0, 1e-4, 1e-4
-    std = torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(DEV)
-    A6 = [35 / 384, 0.0, 500 / 1113, 125 / 192, -2187 / 6784, 11 / 84]
-    E = [35 / 384 - 1951 / 21600, 0.0, 500 / 1113 - 22642 / 50085, 125 / 192 - 451 / 720,
-         -2187 / 6784 + 12231 / 42400, 11 / 84 - 649 / 6300]
-    xd, kd = x.to(DEV), k.to(DEV).contiguous()
-    xnew, errp = torch.zeros(B, D, device=DEV), torch.zeros(B, D, device=DEV)
-    m.vector_field_rkstage(std, xd, kd, 6, xnew, errp)
-    xs = x.double() + 0.125 * sum(a * k[j].double() for j, a in enumerate(A6))
-    ep = sum(e * k[j].double() for j, e in enumerate(E))
-    assert (xnew.cpu().double() - xs).abs().max() <= 4e-6 * xs.abs().max()
-    assert (errp.cpu().double() - ep).abs().max() <= 4e-6 * max(1.0, ep.abs().max().item())
-    ref = f64(0.25 + 1.0 * 0.125, xnew.cpu())
-    got = kd[6].cpu().double()
-    assert (got - ref).abs().max() <= 1e-5 * ref.abs().max()
-    # stage 2 (two derivative arrays, c = 3/10), no side outputs
-    m.vector_field_rkstage(std, xd, kd, 2)
-    xs2 = (x.double() + 0.125 * (3 / 40 * k[0].double() + 9 / 40 * k[1].double())).float()
-    ref2 = f64(float(np.float32(0.25) + np.float32(0.3) * np.float32(0.125)), xs2)
-    assert (kd[2].cpu().double() - ref2).abs().max() <= 1e-5 * ref2.abs().max()
+        assert node.stats["graph"] == graph
+    (o_g, s_g), (o_e, s_e) = outs
+    assert torch.equal(o_g, o_e)
+    assert (s_g["nfe"], s_g["accepted"], s_g["rejected"], s_g["last_ratio"]) == \
+        (s_e["nfe"], s_e["accepted"], s_e["rejected"], s_e["last_ratio"])
 
 
 # ------------------------------------------------- float64-potential Sinkhorn with fp32 screening (BASELINE config 4)

@@ -309,8 +309,8 @@ def _eval_c_fraction_table(text):
 
 
 def test_rk_tableau_header_is_the_oracles_dormand_prince_tableau():
-    """csrc/rk_tableau.h feeds both rk.cu's device constants and the stage row cfm_mlp_forward_rkstage_f32 hands to the
-    fused MLP kernel: every coefficient equals the oracle's (SciPy-pinned) Dormand-Prince tableau rounded to fp32."""
+    """csrc/rk_tableau.h feeds rk.cu's device constants and its compile-time stage rows: every coefficient equals the
+    oracle's (SciPy-pinned) Dormand-Prince tableau rounded to fp32."""
     import re
     from oracle import vector_field as vf
     src = open(os.path.join(ROOT, "cfm_b200", "csrc", "rk_tableau.h")).read()
