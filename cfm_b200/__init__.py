@@ -15,7 +15,7 @@ from .conditional_flow_matching import (ConditionalFlowMatcher,  # noqa: F401
                                         SchrodingerBridgeConditionalFlowMatcher,
                                         TargetConditionalFlowMatcher,
                                         VariancePreservingConditionalFlowMatcher, pad_t_like_x)
-from .models import MLP, torch_wrapper  # noqa: F401
+from .models import MLP, cnf_wrapper, torch_wrapper  # noqa: F401
 from .ode import NeuralODE  # noqa: F401
 from .optimal_transport import CouplingStream, OTPlanSampler, wasserstein  # noqa: F401
 

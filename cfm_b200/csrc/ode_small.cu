@@ -27,6 +27,12 @@
 // a K-split variant in which four warps share a row pair (a quarter of every layer's inputs each, partial sums
 // met behind 128-thread named barriers: 5x fewer instructions per warp, but four barriers per evaluation and the
 // Runge-Kutta arithmetic of a 2-D state serialised in one warp ate the gain).
+//
+// CNF variant (CNF = true; the exact-likelihood field of cnf_wrapper, DESIGN.md section 3.8): the state row is
+// [x, ll] (dim + 1 floats) and the field is [f(t, x), tr(df/dx)].  mlp_eval carries dim forward-mode tangents
+// T_k = dh/dx_k next to the activations: registers for the lane's own units, the per-warp hidden buffers for
+// layer inputs (hbuf grows by 1 + dim).  The f part runs exactly the instructions of the plain variant, so the
+// x columns are bit-identical to it; the trace costs about dim more forwards per evaluation.
 #include <cooperative_groups.h>
 
 #include "mlp_common.cuh"
@@ -61,7 +67,7 @@ struct OdeSmallParams {
   int n_span;
   float atol, rtol;
   int solver;  // 0 dopri5, 1 euler
-  float* traj;  // [n_span][B][dim]
+  float* traj;  // [n_span][B][dim] ([n_span][B][dim + 1] for the CNF variant; so is x0)
   cfm_rk_state* st;
   double* partials;  // [2][3][gridDim.x]
   int rows_per_warp;
@@ -75,9 +81,10 @@ struct SmemPlan {
   int dimp;
   size_t wt0, wtime, b0, wt1, b1, wt2, b2, wt3, b3, hbuf, xin, state, red, total;  // float offsets / bytes
 };
-__host__ __device__ inline SmemPlan ode_small_plan(int dim, int w, int nwarps, int rpw) {
+// cnf: the state row has dim + 1 columns and each hidden buffer row carries dim tangent rows after it
+__host__ __device__ inline SmemPlan ode_small_plan(int dim, int w, int nwarps, int rpw, bool cnf = false) {
   SmemPlan s;
-  s.dimp = (dim + 3) / 4 * 4;
+  s.dimp = (dim + (cnf ? 1 : 0) + 3) / 4 * 4;
   size_t o = 0;
   auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };
   s.wt0 = take((size_t)dim * w);
@@ -89,7 +96,7 @@ __host__ __device__ inline SmemPlan ode_small_plan(int dim, int w, int nwarps, i
   s.b2 = take(w);
   s.wt3 = take((size_t)w * dim);
   s.b3 = take(dim);
-  s.hbuf = take((size_t)nwarps * RB * 2 * w);
+  s.hbuf = take((size_t)nwarps * RB * 2 * w * (cnf ? 1 + dim : 1));
   s.xin = take((size_t)nwarps * RB * s.dimp);
   s.state = take((size_t)nwarps * rpw * kSlots * s.dimp);
   s.red = take(2 * 3 * 32 + 8);  // doubles: 3 x 32 per-warp partials + 3 totals
@@ -111,17 +118,32 @@ __device__ __forceinline__ void sts_units(float* p, const float (&v)[U]) {
   else { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
 }
 
+// d act / dx at the pre-activation x, from the same ex2 approximation act_apply_fast uses
+__device__ __forceinline__ float act_deriv_fast(float x, int act) {
+  if (act == CFM_ACT_SELU) {
+    const float scale = 1.0507009873554804934193349852946f;
+    const float negcoef = (float)(1.6732632423543772848170429916717 * 1.0507009873554804934193349852946);
+    return x > 0.f ? scale : ex2f(x * kLog2e) * negcoef;
+  }
+  const float s = __fdividef(1.f, 1.f + ex2f(-x * kLog2e));  // SiLU' = s + x s (1 - s), s = sigmoid(x)
+  return fmaf(x * s, 1.f - s, s);
+}
+
 // One MLP evaluation f(t, x) for RB rows at once: x_r = xin0 / xin1 -> out0 / out1 (shared memory, dim
 // floats each).  hA, hB: per-warp hidden buffers, [RB][W] each.
+// CNF: out_r also receives div_r = tr(df/dx) at [dim]; hA, hB are [RB][W] activations followed by [RB][dim][W]
+// tangents, and dim <= 8 (the layer-3 branch that ends in a warp reduction).
 // Deliberately NOT inlined and with rolled loops: the kernel runs 1-2 warps per scheduler, and
 // straight-line code of a few thousand instructions would not stay in the instruction cache.
-template <int U>
+template <int U, bool CNF>
 __device__ __noinline__ void mlp_eval(const float* __restrict__ sm, const SmemPlan& pl, int dim, int tv, int act,
                                       const float* xin0, const float* xin1, float t, float* hA, float* hB,
                                       float* out0, float* out1, int lane) {
   constexpr int W = 32 * U;
   const int u0 = U * lane;
   float acc[RB][U], wv[U];
+  [[maybe_unused]] float dact[RB][U];        // CNF: act'(pre-activation) of this lane's units
+  [[maybe_unused]] float dv[RB] = {0.f, 0.f};  // CNF: this lane's share of the divergence
   // layer 0: dim (+ time) -> W
   lds_units<U>(sm + pl.b0 + u0, acc[0]);
   if (tv) {
@@ -143,9 +165,26 @@ __device__ __noinline__ void mlp_eval(const float* __restrict__ sm, const SmemPl
   }
 #pragma unroll
   for (int r = 0; r < RB; ++r) {
+    if constexpr (CNF) {
+#pragma unroll
+      for (int q = 0; q < U; ++q) dact[r][q] = act_deriv_fast(acc[r][q], act);
+    }
 #pragma unroll
     for (int q = 0; q < U; ++q) acc[r][q] = act_apply_fast(acc[r][q], act);
     sts_units<U>(hA + r * W + u0, acc[r]);
+  }
+  if constexpr (CNF) {
+    // layer-0 tangents: T_k = act'(pre0) * W0x[:, k] (the time column does not depend on x)
+    for (int k = 0; k < dim; ++k) {
+      lds_units<U>(sm + pl.wt0 + (size_t)k * W + u0, wv);
+#pragma unroll
+      for (int r = 0; r < RB; ++r) {
+        float tk[U];
+#pragma unroll
+        for (int q = 0; q < U; ++q) tk[q] = dact[r][q] * wv[q];
+        sts_units<U>(hA + (RB + r * dim + k) * W + u0, tk);
+      }
+    }
   }
   __syncwarp();
   // layers 1, 2: W -> W
@@ -175,9 +214,56 @@ __device__ __noinline__ void mlp_eval(const float* __restrict__ sm, const SmemPl
     }
 #pragma unroll
     for (int r = 0; r < RB; ++r) {
+      if constexpr (CNF) {
+#pragma unroll
+        for (int q = 0; q < U; ++q) dact[r][q] = act_deriv_fast(acc[r][q], act);
+      }
 #pragma unroll
       for (int q = 0; q < U; ++q) acc[r][q] = act_apply_fast(acc[r][q], act);
       sts_units<U>(hout + r * W + u0, acc[r]);
+    }
+    if constexpr (CNF) {
+      // tangents: T_k <- act'(pre) * (W T_k), one weight pass per input direction k
+      for (int k = 0; k < dim; ++k) {
+        const float* ta = hin + (RB + k) * W;
+        const float* tb = hin + (RB + dim + k) * W;
+        float tk[RB][U];
+#pragma unroll
+        for (int r = 0; r < RB; ++r)
+#pragma unroll
+          for (int q = 0; q < U; ++q) tk[r][q] = 0.f;
+#pragma unroll 2
+        for (int i = 0; i < W; i += 4) {
+          const float4 va = *reinterpret_cast<const float4*>(ta + i);
+          const float4 vb = *reinterpret_cast<const float4*>(tb + i);
+          const float ts[RB][4] = {{va.x, va.y, va.z, va.w}, {vb.x, vb.y, vb.z, vb.w}};
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            lds_units<U>(wt + (size_t)(i + c) * W + u0, wv);
+#pragma unroll
+            for (int q = 0; q < U; ++q) {
+              tk[0][q] = fmaf(wv[q], ts[0][c], tk[0][q]);
+              tk[1][q] = fmaf(wv[q], ts[1][c], tk[1][q]);
+            }
+          }
+        }
+#pragma unroll
+        for (int r = 0; r < RB; ++r)
+#pragma unroll
+          for (int q = 0; q < U; ++q) tk[r][q] *= dact[r][q];
+        if (layer == 0) {
+#pragma unroll
+          for (int r = 0; r < RB; ++r) sts_units<U>(hout + (RB + r * dim + k) * W + u0, tk[r]);
+        } else {
+          // last hidden layer: only (W3 T_k)_k enters the trace, so fold row k of W3 in here
+#pragma unroll
+          for (int q = 0; q < U; ++q) {
+            const float w3 = sm[pl.wt3 + (size_t)(u0 + q) * dim + k];
+            dv[0] = fmaf(w3, tk[0][q], dv[0]);
+            dv[1] = fmaf(w3, tk[1][q], dv[1]);
+          }
+        }
+      }
     }
     __syncwarp();
   }
@@ -200,6 +286,17 @@ __device__ __noinline__ void mlp_eval(const float* __restrict__ sm, const SmemPl
         const float b3 = sm[pl.b3 + e];
         out0[e] = pa + b3;
         out1[e] = pb + b3;
+      }
+    }
+    if constexpr (CNF) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        dv[0] += __shfl_xor_sync(0xffffffffu, dv[0], o);
+        dv[1] += __shfl_xor_sync(0xffffffffu, dv[1], o);
+      }
+      if (lane == 0) {
+        out0[dim] = dv[0];
+        out1[dim] = dv[1];
       }
     }
   } else {
@@ -259,14 +356,15 @@ __device__ __noinline__ void grid_sum(cg::grid_group& grid, double (&v)[NV], dou
   __syncthreads();  // red is reused by the next call
 }
 
-template <int U, int MAXT>
+template <int U, int MAXT, bool CNF>
 __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams p) {
   constexpr int W = 32 * U;
   extern __shared__ __align__(16) float sm[];
   cg::grid_group grid = cg::this_grid();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
   const int dim = p.dim, tv = p.tv, act = p.act, rpw = p.rows_per_warp;
-  const SmemPlan pl = ode_small_plan(dim, W, nwarps, rpw);
+  const int sw = CNF ? dim + 1 : dim;  // state columns: x (and the log-density column ll)
+  const SmemPlan pl = ode_small_plan(dim, W, nwarps, rpw, CNF);
   const int dimp = pl.dimp;
   const int in0 = dim + tv;
 
@@ -292,8 +390,9 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
   }
   for (int e = tid; e < dim; e += blockDim.x) sm[pl.b3 + e] = p.b3[e];
 
-  float* hA = sm + pl.hbuf + (size_t)warp * RB * 2 * W;  // [RB][W]
-  float* hB = hA + RB * W;                                // [RB][W]
+  const int hsz = CNF ? RB * W * (1 + dim) : RB * W;     // one hidden buffer: [RB][W] (+ [RB][dim][W] tangents)
+  float* hA = sm + pl.hbuf + (size_t)warp * 2 * hsz;
+  float* hB = hA + hsz;
   float* xin = sm + pl.xin + (size_t)warp * RB * dimp;    // [RB][dimp]
   double* red = reinterpret_cast<double*>(sm + pl.red);
   const int64_t gwarp = (int64_t)blockIdx.x * nwarps + warp, wstride = (int64_t)gridDim.x * nwarps;
@@ -301,15 +400,15 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
   auto row_of = [&](int j) -> int64_t { return (gwarp + (int64_t)(j / RB) * wstride) * RB + (j % RB); };
   auto slot = [&](int j, int s) -> float* { return sm + pl.state + (((size_t)warp * rpw + j) * kSlots + s) * dimp; };
   const int64_t B = p.B;
-  const double numel = (double)B * (double)dim;
+  const double numel = (double)B * (double)sw;
 
   // ---- x0 -> state (rows past the batch: zeros, integrated along but never stored or counted), traj[0] ----
   for (int j = 0; j < rpw; ++j) {
     const int64_t r = row_of(j);
-    for (int e = lane; e < dim; e += 32) {
-      const float v = r < B ? p.x0[r * dim + e] : 0.f;
+    for (int e = lane; e < sw; e += 32) {
+      const float v = r < B ? p.x0[r * sw + e] : 0.f;
       slot(j, 0)[e] = v;
-      if (r < B) p.traj[r * dim + e] = v;
+      if (r < B) p.traj[r * sw + e] = v;
     }
   }
   __syncthreads();
@@ -321,16 +420,16 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
       const float t = __ldg(p.t_span + n), h = __ldg(p.t_span + n + 1) - t;
       for (int g = 0; g < rpw; g += RB) {
         if (row_of(g) >= B) break;
-        mlp_eval<U>(sm, pl, dim, tv, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 1), slot(g + 1, 1), lane);
+        mlp_eval<U, CNF>(sm, pl, dim, tv, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 1), slot(g + 1, 1), lane);
 #pragma unroll
         for (int m = 0; m < RB; ++m) {
           const int64_t r = row_of(g + m);
           float* x = slot(g + m, 0);
           const float* k = slot(g + m, 1);
-          for (int e = lane; e < dim; e += 32) {
+          for (int e = lane; e < sw; e += 32) {
             const float v = fmaf(h, k[e], x[e]);
             x[e] = v;
-            if (r < B) p.traj[((int64_t)(n + 1) * B + r) * dim + e] = v;
+            if (r < B) p.traj[((int64_t)(n + 1) * B + r) * sw + e] = v;
           }
         }
         __syncwarp();
@@ -368,11 +467,11 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
     double s2[2] = {0.0, 0.0};
     for (int g = 0; g < rpw; g += RB) {
       if (row_of(g) >= B) break;
-      mlp_eval<U>(sm, pl, dim, tv, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 1), slot(g + 1, 1), lane);
+      mlp_eval<U, CNF>(sm, pl, dim, tv, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 1), slot(g + 1, 1), lane);
 #pragma unroll
       for (int m = 0; m < RB; ++m) {
         if (row_of(g + m) >= B) continue;
-        for (int e = lane; e < dim; e += 32) {
+        for (int e = lane; e < sw; e += 32) {
           const float xv = slot(g + m, 0)[e], f0 = slot(g + m, 1)[e];
           const float sc = atol + fabsf(xv) * rtol;
           const float a = xv / sc, b = f0 / sc;
@@ -390,13 +489,13 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
       if (row_of(g) >= B) break;
 #pragma unroll
       for (int m = 0; m < RB; ++m)
-        for (int e = lane; e < dim; e += 32) xin[m * dimp + e] = fmaf(h0, slot(g + m, 1)[e], slot(g + m, 0)[e]);
+        for (int e = lane; e < sw; e += 32) xin[m * dimp + e] = fmaf(h0, slot(g + m, 1)[e], slot(g + m, 0)[e]);
       __syncwarp();
-      mlp_eval<U>(sm, pl, dim, tv, act, xin, xin + dimp, t + h0, hA, hB, slot(g, 2), slot(g + 1, 2), lane);
+      mlp_eval<U, CNF>(sm, pl, dim, tv, act, xin, xin + dimp, t + h0, hA, hB, slot(g, 2), slot(g + 1, 2), lane);
 #pragma unroll
       for (int m = 0; m < RB; ++m) {
         if (row_of(g + m) >= B) continue;
-        for (int e = lane; e < dim; e += 32) {
+        for (int e = lane; e < sw; e += 32) {
           const float sc = atol + fabsf(slot(g + m, 0)[e]) * rtol;
           const float q = (slot(g + m, 2)[e] - slot(g + m, 1)[e]) / sc;
           s1[0] += (double)q * q;
@@ -432,7 +531,7 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
         for (int m = 0; m < RB; ++m) {
           float* dst = m == 0 ? d0p : d1p;
           const float* x = slot(g + m, 0);
-          for (int e = lane; e < dim; e += 32) {
+          for (int e = lane; e < sw; e += 32) {
             float v = x[e];
 #pragma unroll
             for (int q = 0; q < 6; ++q)
@@ -441,14 +540,14 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
           }
         }
         __syncwarp();
-        mlp_eval<U>(sm, pl, dim, tv, act, d0p, d1p, t + oC[stage] * dt, hA, hB, slot(g, 1 + stage),
+        mlp_eval<U, CNF>(sm, pl, dim, tv, act, d0p, d1p, t + oC[stage] * dt, hA, hB, slot(g, 1 + stage),
                     slot(g + 1, 1 + stage), lane);
       }
 #pragma unroll
       for (int m = 0; m < RB; ++m) {
         if (row_of(g + m) >= B) continue;
         const float* x = slot(g + m, 0);
-        for (int e = lane; e < dim; e += 32) {
+        for (int e = lane; e < sw; e += 32) {
           float er = 0.f;
 #pragma unroll
           for (int q = 0; q < 7; ++q)
@@ -495,11 +594,11 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
       for (int j = 0; j < rpw; ++j) {
         const int64_t r = row_of(j);
         if (r >= B) break;
-        for (int e = lane; e < dim; e += 32) {
+        for (int e = lane; e < sw; e += 32) {
           const float v = slot(j, 8)[e];
           slot(j, 0)[e] = v;
           slot(j, 1)[e] = slot(j, 7)[e];
-          if (save_slot >= 0) p.traj[((int64_t)save_slot * B + r) * dim + e] = v;
+          if (save_slot >= 0) p.traj[((int64_t)save_slot * B + r) * sw + e] = v;
         }
       }
       __syncwarp();
@@ -519,36 +618,54 @@ struct Launch {
   size_t smem;
 };
 
+// CNF: at most this many warps per CTA.  With the tangent loops the kernel spills at the 128 registers per thread
+// that 512-thread launch bounds leave, and not at 256 threads (ptxas -v).
+constexpr int kCnfMaxWarps = 8;
+
 template <int U>
-int plan_launch(int64_t B, int dim, Launch* out) {
+int plan_launch(int64_t B, int dim, bool cnf, Launch* out) {
   const int sms = sm_count();
   const int64_t groups = (B + RB - 1) / RB;  // a warp integrates RB rows at a time
-  for (int nwarps = 4; nwarps <= 32; nwarps *= 2) {
-    int64_t grid = (groups + nwarps - 1) / nwarps;
+  const int max_warps = cnf ? kCnfMaxWarps : 32;
+  int64_t grid = 0, gpw = 0;
+  auto shape = [&](int nwarps) {
+    grid = (groups + nwarps - 1) / nwarps;
     if (grid > sms) grid = sms;
     const int64_t per = grid * nwarps;
-    const int64_t gpw = (groups + per - 1) / per;  // groups per warp
-    if (gpw > 1 && nwarps < 32) continue;  // prefer more warps per CTA over several groups per warp
-    if (gpw > (1 << 19)) return 0;
-    const SmemPlan pl = ode_small_plan(dim, 32 * U, nwarps, (int)gpw * RB);
-    if (pl.total > 200 * 1024) return 0;
-    out->grid = (int)grid; out->nwarps = nwarps; out->rpw = (int)gpw * RB; out->smem = pl.total;
-    return 1;
+    gpw = (groups + per - 1) / per;  // groups per warp
+  };
+  int nwarps = 4;
+  for (;; nwarps *= 2) {  // prefer more warps per CTA over several groups per warp
+    shape(nwarps);
+    if (gpw == 1 || nwarps == max_warps) break;
   }
-  return 0;
+  for (;;) {
+    if (gpw > (1 << 19)) return 0;
+    const SmemPlan pl = ode_small_plan(dim, 32 * U, nwarps, (int)gpw * RB, cnf);
+    if (pl.total <= 200 * 1024) {
+      out->grid = (int)grid; out->nwarps = nwarps; out->rpw = (int)gpw * RB; out->smem = pl.total;
+      return 1;
+    }
+    // CNF: the tangent buffers grow with the warps per CTA while the per-CTA row state does not, so fewer warps
+    // with more row groups each may still fit
+    if (!cnf || nwarps == 4) return 0;
+    nwarps /= 2;
+    shape(nwarps);
+  }
 }
 
-int plan_any(int64_t B, int dim, int w, Launch* out) {
+int plan_any(int64_t B, int dim, int w, Launch* out, bool cnf = false) {
   if (B <= 0 || dim <= 0 || dim > 1024) return 0;
-  if (w == 32) return plan_launch<1>(B, dim, out);
-  if (w == 64) return plan_launch<2>(B, dim, out);
-  if (w == 128) return plan_launch<4>(B, dim, out);
+  if (cnf && dim > 8) return 0;  // the exact trace takes the layer-3 branch that ends in a warp reduction
+  if (w == 32) return plan_launch<1>(B, dim, cnf, out);
+  if (w == 64) return plan_launch<2>(B, dim, cnf, out);
+  if (w == 128) return plan_launch<4>(B, dim, cnf, out);
   return 0;
 }
 
-template <int U, int MAXT>
+template <int U, int MAXT, bool CNF>
 int launch_t(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {
-  const void* kern = (const void*)ode_small_kernel<U, MAXT>;
+  const void* kern = (const void*)ode_small_kernel<U, MAXT, CNF>;
   CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
   int per_sm = 0;
   CFM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, L.nwarps * 32, L.smem));
@@ -560,9 +677,45 @@ int launch_t(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {
 }
 template <int U>
 int launch(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {
-  if (L.nwarps <= 8) return launch_t<U, 256>(p, L, s);
-  if (L.nwarps <= 16) return launch_t<U, 512>(p, L, s);
-  return launch_t<U, 1024>(p, L, s);
+  if (L.nwarps <= 8) return launch_t<U, 256, false>(p, L, s);
+  if (L.nwarps <= 16) return launch_t<U, 512, false>(p, L, s);
+  return launch_t<U, 1024, false>(p, L, s);
+}
+template <int U>
+int launch_cnf(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {
+  static_assert(kCnfMaxWarps <= 8, "the CNF variant is instantiated for 256-thread CTAs only");
+  return launch_t<U, 256, true>(p, L, s);
+}
+
+int trajectory(bool cnf, const char* what, const float* W0, const float* b0, const float* W1, const float* b1,
+               const float* W2, const float* b2, const float* W3, const float* b3, int dim, int w, int time_varying,
+               int act, const float* x0, int64_t batch, const float* t_span, int n_span, float atol, float rtol,
+               int solver, float* traj, cfm_rk_state* state_out, void* workspace, size_t workspace_bytes,
+               void* stream) {
+  CFM_REQUIRE(W0 && b0 && W1 && b1 && W2 && b2 && W3 && b3 && x0 && t_span && traj && state_out && workspace,
+              "%s: null pointer", what);
+  CFM_REQUIRE(n_span >= 2 && (solver == 0 || solver == 1) && (act == CFM_ACT_SELU || act == CFM_ACT_SILU),
+              "%s: bad argument", what);
+  CFM_REQUIRE(workspace_bytes >= cfm_ode_small_workspace_bytes(batch, dim, w), "%s: workspace too small", what);
+  Launch L;
+  CFM_REQUIRE(plan_any(batch, dim, w, &L, cnf), "%s: unsupported shape B=%lld dim=%d w=%d", what, (long long)batch,
+              dim, w);
+  OdeSmallParams p;
+  p.W0 = W0; p.b0 = b0; p.W1 = W1; p.b1 = b1; p.W2 = W2; p.b2 = b2; p.W3 = W3; p.b3 = b3;
+  p.dim = dim; p.w = w; p.tv = time_varying ? 1 : 0; p.act = act;
+  p.x0 = x0; p.B = batch; p.t_span = t_span; p.n_span = n_span; p.atol = atol; p.rtol = rtol;
+  p.solver = solver; p.traj = traj; p.st = state_out; p.partials = reinterpret_cast<double*>(workspace);
+  p.rows_per_warp = L.rpw; p.max_steps = 1000000;
+  cudaStream_t s = (cudaStream_t)stream;
+  CFM_CUDA_OK(cudaMemsetAsync(state_out, 0, sizeof(cfm_rk_state), s));
+  if (cnf) {
+    if (w == 32) return launch_cnf<1>(p, L, s);
+    if (w == 64) return launch_cnf<2>(p, L, s);
+    return launch_cnf<4>(p, L, s);
+  }
+  if (w == 32) return launch<1>(p, L, s);
+  if (w == 64) return launch<2>(p, L, s);
+  return launch<4>(p, L, s);
 }
 
 }  // namespace
@@ -576,6 +729,11 @@ extern "C" int cfm_ode_small_supported(int64_t batch, int dim, int w, int out_di
   return (out_dim == dim) && plan_any(batch, dim, w, &L);
 }
 
+extern "C" int cfm_ode_small_cnf_supported(int64_t batch, int dim, int w) {
+  Launch L;
+  return plan_any(batch, dim, w, &L, true);
+}
+
 extern "C" size_t cfm_ode_small_workspace_bytes(int64_t batch, int dim, int w) {
   (void)batch; (void)dim; (void)w;
   return align_up((size_t)2 * 3 * (size_t)sm_count() * sizeof(double), 256);
@@ -587,24 +745,18 @@ extern "C" int cfm_ode_small_trajectory_f32(const float* W0, const float* b0, co
                                             const float* t_span, int n_span, float atol, float rtol, int solver,
                                             float* traj, cfm_rk_state* state_out, void* workspace,
                                             size_t workspace_bytes, void* stream) {
-  CFM_REQUIRE(W0 && b0 && W1 && b1 && W2 && b2 && W3 && b3 && x0 && t_span && traj && state_out && workspace,
-              "cfm_ode_small_trajectory_f32: null pointer");
-  CFM_REQUIRE(n_span >= 2 && (solver == 0 || solver == 1) && (act == CFM_ACT_SELU || act == CFM_ACT_SILU),
-              "cfm_ode_small_trajectory_f32: bad argument");
-  CFM_REQUIRE(workspace_bytes >= cfm_ode_small_workspace_bytes(batch, dim, w),
-              "cfm_ode_small_trajectory_f32: workspace too small");
-  Launch L;
-  CFM_REQUIRE(plan_any(batch, dim, w, &L), "cfm_ode_small_trajectory_f32: unsupported shape B=%lld dim=%d w=%d",
-              (long long)batch, dim, w);
-  OdeSmallParams p;
-  p.W0 = W0; p.b0 = b0; p.W1 = W1; p.b1 = b1; p.W2 = W2; p.b2 = b2; p.W3 = W3; p.b3 = b3;
-  p.dim = dim; p.w = w; p.tv = time_varying ? 1 : 0; p.act = act;
-  p.x0 = x0; p.B = batch; p.t_span = t_span; p.n_span = n_span; p.atol = atol; p.rtol = rtol;
-  p.solver = solver; p.traj = traj; p.st = state_out; p.partials = reinterpret_cast<double*>(workspace);
-  p.rows_per_warp = L.rpw; p.max_steps = 1000000;
-  cudaStream_t s = (cudaStream_t)stream;
-  CFM_CUDA_OK(cudaMemsetAsync(state_out, 0, sizeof(cfm_rk_state), s));
-  if (w == 32) return launch<1>(p, L, s);
-  if (w == 64) return launch<2>(p, L, s);
-  return launch<4>(p, L, s);
+  return trajectory(false, "cfm_ode_small_trajectory_f32", W0, b0, W1, b1, W2, b2, W3, b3, dim, w, time_varying,
+                    act, x0, batch, t_span, n_span, atol, rtol, solver, traj, state_out, workspace, workspace_bytes,
+                    stream);
+}
+
+extern "C" int cfm_ode_small_cnf_trajectory_f32(const float* W0, const float* b0, const float* W1, const float* b1,
+                                                const float* W2, const float* b2, const float* W3, const float* b3,
+                                                int dim, int w, int time_varying, int act, const float* x0,
+                                                int64_t batch, const float* t_span, int n_span, float atol,
+                                                float rtol, int solver, float* traj, cfm_rk_state* state_out,
+                                                void* workspace, size_t workspace_bytes, void* stream) {
+  return trajectory(true, "cfm_ode_small_cnf_trajectory_f32", W0, b0, W1, b1, W2, b2, W3, b3, dim, w,
+                    time_varying, act, x0, batch, t_span, n_span, atol, rtol, solver, traj, state_out, workspace,
+                    workspace_bytes, stream);
 }

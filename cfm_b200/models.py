@@ -32,6 +32,7 @@ class MLP(torch.nn.Module):
         self.act = _ffi.ACT_SELU
         self.mlp_algo = 0  # 0 auto, 1 SIMT fp32, 2 tensor cores (fp16x3 scheme: fused kernel for w = 256, per-layer otherwise)
         self._blobs = {}   # (split_t, device) -> (version key, prepared blob tensor)
+        self._reversed = None  # (version key, time-reversed MLP); a tuple, so it is not registered as a submodule
 
     # -- prepared weights (rebuilt when any parameter changes in place or is replaced) ------
     def _linears(self):
@@ -67,6 +68,30 @@ class MLP(torch.nn.Module):
                        "cfm_mlp_prepare")
         self._blobs[key] = (ver, blob)
         return blob
+
+    def _time_reversed(self):
+        """The field f_(s, x) = -f(-s, x) as an MLP: W3, b3 and the time column of W0 negated.  A decreasing
+        ``t_span`` is integrated as this field over ``-t_span`` (torchdyn's reparametrisation); negation is exact
+        and fmaf(-s, -w, b) == fmaf(s, w, b), so the time input keeps its bits.  Built once per weight version."""
+        if not self.time_varying:
+            raise RuntimeError("a time-reversed field needs an MLP built with time_varying=True")
+        ver = self._weights_key()
+        hit = getattr(self, "_reversed", None)  # absent on modules pickled before the cache existed
+        if hit is not None and hit[0] == ver:
+            m = hit[1]
+        else:
+            w0 = self.net[0].weight
+            m = MLP(self.dim, self.out_dim, self.w, self.time_varying).to(device=w0.device, dtype=w0.dtype)
+            with torch.no_grad():
+                for dst, src in zip(m._linears(), self._linears()):
+                    dst.weight.copy_(src.weight)
+                    dst.bias.copy_(src.bias)
+                m.net[0].weight[:, -1].neg_()
+                m.net[6].weight.neg_()
+                m.net[6].bias.neg_()
+            self._reversed = (ver, m)
+        m.act, m.mlp_algo = self.act, self.mlp_algo
+        return m
 
     def _kernel_forward(self, x, t_dev, t_host, split_t, out=None):
         L = _ffi.lib()
@@ -156,3 +181,68 @@ class torch_wrapper(torch.nn.Module):
         if isinstance(self.model, MLP) and self.model.time_varying and self.model._use_kernels(x):
             return self.model.vector_field(t, x)
         return self.model(torch.cat([x, t.repeat(x.shape[0])[:, None]], 1))
+
+
+def exact_div_fn(u):
+    """div u = tr(du/dy) of a map u: R^D -> R^D at one point, from its full Jacobian (torch.func.jacrev)."""
+    jac = torch.func.jacrev(u)
+
+    def div(y, *args):
+        return torch.trace(jac(y))
+
+    return div
+
+
+def div_fn_hutch_trace(u):
+    """Hutchinson's estimate eps . (du/dy)^T eps of div u at one point, from one vector-Jacobian product."""
+    def div(y, eps):
+        _, pullback = torch.func.vjp(u, y)
+        return (pullback(eps)[0] * eps).sum()
+
+    return div
+
+
+def _rademacher_like(x):
+    return torch.randint_like(x, low=0, high=2).float() * 2 - 1.0
+
+
+class cnf_wrapper(torch.nn.Module):
+    """Continuous-normalising-flow field of the maximum-likelihood tutorial
+    (examples/2D_tutorials/Maximum_likelihood_CNF_tutorial.ipynb): the state is [x, ll] with the log-density change
+    as its LAST column, and d/dt [x, ll] = [f(t, x), div f(t, x)].  Integrating [x1, 0] from t = 1 to t = 0 gives
+    log p(x1) = prior.log_prob(x0) + ll.
+
+    ``forward(t, x)`` is plain PyTorch (torch.func per row), so maximum-likelihood training backpropagates through it
+    on any device.  Under ``torch.no_grad()`` on CUDA, ``cfm_b200.NeuralODE`` integrates a wrapped
+    ``MLP(time_varying=True)`` with ``likelihood_estimator="exact"`` in one kernel instead (cfm_b200/ode.py)."""
+
+    def __init__(self, model, likelihood_estimator="exact"):
+        super().__init__()
+        self.model = model
+        self.likelihood_estimator = likelihood_estimator
+        self.div_fn, self.eps_fn = self.get_div_and_eps(likelihood_estimator)
+
+    def get_div_and_eps(self, likelihood_estimator):
+        """(divergence-function factory, probe-vector sampler or None) for an estimator name."""
+        if likelihood_estimator == "exact":
+            return exact_div_fn, None
+        if likelihood_estimator == "hutch_gaussian":
+            return div_fn_hutch_trace, torch.randn_like
+        if likelihood_estimator == "hutch_rademacher":
+            return div_fn_hutch_trace, _rademacher_like
+        raise NotImplementedError(f"likelihood estimator {likelihood_estimator} is not implemented")
+
+    def forward(self, t, x, *args, **kwargs):
+        t = t.squeeze()
+        x = x[..., :-1]
+
+        def field(y):  # one row: u(y) = model([y, t])
+            return self.model(torch.cat([y, t[None]]))
+
+        div_fn = self.div_fn(field)
+        if self.eps_fn is None:
+            div = torch.vmap(div_fn)(x)
+        else:
+            div = torch.vmap(div_fn)(x, self.eps_fn(x))
+        dx = self.model(torch.cat([x, t.repeat(x.shape[0])[:, None]], 1))
+        return torch.cat([dx, div[:, None]], dim=-1)

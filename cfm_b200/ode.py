@@ -15,14 +15,20 @@ whether the integration has finished.
 
 Only the hot path the north_star names is accelerated: the vector field must be a
 ``cfm_b200.models.MLP`` (optionally inside ``torch_wrapper``) on a CUDA device; anything else
-raises -- there is no eager fallback.
+raises -- there is no eager fallback.  ``cnf_wrapper(MLP(time_varying=True), "exact")`` is accepted too: its
+state carries the log-density column, and the whole trajectory, trace included, runs in the one-launch kernel
+(csrc/ode_small.cu, CNF variant).
+
+A decreasing ``t_span`` is integrated as torchdyn does: dopri5 runs the field f_(s, x) = -f(-s, x) over
+s = -t_span (for the MLP only a different weight set, ``MLP._time_reversed``), because the step controller
+only steps forwards.  Euler needs no such step: a negative step already gives the same bits.
 """
 import ctypes as C
 
 import torch
 
 from . import _ffi
-from .models import MLP, torch_wrapper
+from .models import MLP, cnf_wrapper, torch_wrapper
 
 
 def _unwrap(vf):
@@ -32,6 +38,23 @@ def _unwrap(vf):
                         "vector fields (optionally wrapped in torch_wrapper); got "
                         f"{type(m).__name__}")
     return m
+
+
+def _unwrap_cnf(vf):
+    if vf.eps_fn is not None:
+        raise NotImplementedError(
+            f"cnf_wrapper(likelihood_estimator={vf.likelihood_estimator!r}): the Hutchinson estimators draw their "
+            "probe vectors from torch's RNG on every call, which no device stream reproduces; the CUDA path "
+            "provides the exact trace (likelihood_estimator='exact')")
+    m = vf.model
+    if not isinstance(m, MLP) or not m.time_varying:
+        raise TypeError("cfm_b200.NeuralODE accelerates cnf_wrapper(cfm_b200.models.MLP(time_varying=True)); got "
+                        f"cnf_wrapper({type(m).__name__})")
+    return m
+
+
+def _decreasing(t_span):
+    return t_span.numel() >= 2 and bool(t_span[1] < t_span[0])
 
 
 class NeuralODE(torch.nn.Module):
@@ -67,11 +90,14 @@ class NeuralODE(torch.nn.Module):
 
     @torch.no_grad()
     def trajectory(self, x, t_span):
-        mlp = _unwrap(self.vf)
+        cnf = isinstance(self.vf, cnf_wrapper)
+        mlp = _unwrap_cnf(self.vf) if cnf else _unwrap(self.vf)
         if not x.is_cuda:
             raise _ffi.CfmLibraryError("NeuralODE.trajectory needs CUDA inputs (no CPU fallback)")
         dev = x.device
         with torch.cuda.device(dev):  # the library launches on the CURRENT device: make it the tensors' one
+            if cnf:
+                return self._cnf_trajectory_on(mlp, x, t_span, dev)
             return self._trajectory_on(mlp, x, t_span, dev)
 
     def _trajectory_on(self, mlp, x, t_span, dev):
@@ -80,6 +106,9 @@ class NeuralODE(torch.nn.Module):
         t_span = torch.as_tensor(t_span, dtype=torch.float32)
         if self.lockstep is not None and self.solver != "dopri5":
             raise NotImplementedError("lock-step sharding applies to the adaptive solver (dopri5)")
+        reverse = self.solver == "dopri5" and _decreasing(t_span)
+        if reverse:
+            mlp, t_span = mlp._time_reversed(), -t_span
         if self.lockstep is None and self.use_fused_small and t_span.numel() >= 2 \
                 and _ffi.lib().cfm_ode_small_supported(x0.shape[0], x0.shape[1], mlp.w, mlp.out_dim):
             out = self._fused_small(mlp, x0, t_span.to(dev).contiguous())
@@ -89,15 +118,42 @@ class NeuralODE(torch.nn.Module):
             # the span stays on the host (where callers build it): the plan keeps a device copy and refreshes it only
             # when the values change, so a repeated call neither uploads nor reads back anything before the first kernel
             out = self._dopri5(mlp, x0, t_span.detach().cpu().contiguous())
+        if reverse:
+            self.stats["t"] = -self.stats["t"]
         return out.reshape(out.shape[0], *shape)
 
+    def _cnf_trajectory_on(self, mlp, x, t_span, dev):
+        """cnf_wrapper(mlp, "exact"): the state [x, ll] goes through the CNF variant of the one-launch kernel."""
+        if self.lockstep is not None:
+            raise NotImplementedError("cnf_wrapper: lock-step sharding is not supported; the exact-likelihood path "
+                                      "integrates the whole batch in one single-device kernel")
+        if x.dim() != 2 or x.shape[1] != mlp.dim + 1:
+            raise ValueError(f"cnf_wrapper: expected a state of shape (B, {mlp.dim + 1}) (x and the log-density "
+                             f"column), got {tuple(x.shape)}")
+        t_span = torch.as_tensor(t_span, dtype=torch.float32)
+        if t_span.numel() < 2:
+            raise ValueError("cnf_wrapper: t_span needs at least two points")
+        if mlp.out_dim != mlp.dim or not _ffi.lib().cfm_ode_small_cnf_supported(x.shape[0], mlp.dim, mlp.w):
+            raise NotImplementedError(
+                f"cnf_wrapper: no exact-likelihood kernel for B={x.shape[0]}, dim={mlp.dim}, w={mlp.w}, "
+                f"out_dim={mlp.out_dim} (it takes w in {{32, 64, 128}}, dim <= 8, out_dim == dim and batches whose "
+                "state fits in shared memory)")
+        reverse = self.solver == "dopri5" and _decreasing(t_span)
+        if reverse:
+            mlp, t_span = mlp._time_reversed(), -t_span
+        out = self._fused_small(mlp, x.detach().float().contiguous(), t_span.to(dev).contiguous(), cnf=True)
+        if reverse:
+            self.stats["t"] = -self.stats["t"]
+        return out
+
     # ------------------------------------------------------------------------------------
-    def _fused_small(self, mlp, x0, t_span):
+    def _fused_small(self, mlp, x0, t_span, cnf=False):
         """Launch-bound regime (the 2-D tutorial models): Hairer init, all dopri5 / euler steps, the
-        error norms and the controller in ONE cooperative kernel; one host read at the end."""
+        error norms and the controller in ONE cooperative kernel; one host read at the end.  ``cnf``: x0 is the
+        [x, ll] state of cnf_wrapper (mlp.dim + 1 columns) and the kernel also integrates the trace."""
         L = _ffi.lib()
         dev = x0.device
-        B, D = x0.shape
+        B, D = x0.shape  # D: state columns
         n_span = t_span.numel()
         ps = []
         for lin in mlp._linears():
@@ -107,11 +163,13 @@ class NeuralODE(torch.nn.Module):
                 ps.append(p.detach().contiguous())
         traj = torch.empty((n_span, B, D), dtype=torch.float32, device=dev)
         st = torch.zeros(ctypes_sizeof_state(), dtype=torch.uint8, device=dev)
-        ws = _ffi.workspace(L.cfm_ode_small_workspace_bytes(B, D, mlp.w), dev)
-        _ffi.check(L.cfm_ode_small_trajectory_f32(
-            *[_ffi.ptr(p) for p in ps], D, mlp.w, 1, mlp.act, _ffi.ptr(x0), B, _ffi.ptr(t_span), n_span,
+        dim = mlp.dim if cnf else D
+        ws = _ffi.workspace(L.cfm_ode_small_workspace_bytes(B, dim, mlp.w), dev)
+        name = "cfm_ode_small_cnf_trajectory_f32" if cnf else "cfm_ode_small_trajectory_f32"
+        _ffi.check(getattr(L, name)(
+            *[_ffi.ptr(p) for p in ps], dim, mlp.w, 1, mlp.act, _ffi.ptr(x0), B, _ffi.ptr(t_span), n_span,
             self.atol, self.rtol, 1 if self.solver == "euler" else 0, _ffi.ptr(traj), _ffi.ptr(st),
-            _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)), "cfm_ode_small_trajectory_f32")
+            _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)), name)
         cur = _ffi.RkState.from_buffer_copy(bytes(st.cpu().numpy().tobytes()))
         if not cur.done:
             raise RuntimeError("dopri5: step budget exhausted")

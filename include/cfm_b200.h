@@ -300,6 +300,19 @@ int cfm_ode_small_trajectory_f32(const float* W0, const float* b0, const float* 
                                  int64_t batch, const float* t_span, int n_span, float atol,
                                  float rtol, int solver, float* traj, cfm_rk_state* state_out,
                                  void* workspace, size_t workspace_bytes, void* stream);
+/* Exact-likelihood (CNF) variant of the above: the state is [x, ll] with dim + 1 columns and the field is
+ * [f(t, x), tr(df/dx)] (the log-density column LAST, with +div as its derivative), traced per row by forward-mode
+ * tangents through the same MLP.  x0 is [batch][dim + 1], traj [n_span][batch][dim + 1]; every other argument,
+ * the workspace and the state are as for cfm_ode_small_trajectory_f32, and the error norms cover all
+ * batch * (dim + 1) elements.  supported(): w in {32, 64, 128}, dim <= 8 and the per-row state and tangent
+ * buffers fit in shared memory. */
+int cfm_ode_small_cnf_supported(int64_t batch, int dim, int w);
+int cfm_ode_small_cnf_trajectory_f32(const float* W0, const float* b0, const float* W1, const float* b1,
+                                     const float* W2, const float* b2, const float* W3, const float* b3,
+                                     int dim, int w, int time_varying, int act, const float* x0,
+                                     int64_t batch, const float* t_span, int n_span, float atol,
+                                     float rtol, int solver, float* traj, cfm_rk_state* state_out,
+                                     void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
