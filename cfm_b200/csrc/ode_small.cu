@@ -17,7 +17,7 @@
 //     rows_per_warp rows, whose x, k1..k7 and xnew live in shared memory for the whole trajectory --
 //     HBM is touched only for x0 and for the recorded t_span points;
 //   * the controller is replicated: every thread evaluates the same scalar accept/reject logic
-//     (torchdyn's, as restated in rk.cu) from the same grid-wide error sum, so the only grid-level
+//     (torchdyn's, rk_control.cuh, shared with rk.cu) from the same grid-wide error sum, so the only grid-level
 //     communication is ONE deterministic all-reduce (per-CTA partials -> grid barrier -> every CTA
 //     folds the partials in the same order) per step;
 //   * solver = euler needs no barrier at all.
@@ -36,6 +36,8 @@
 #include <cooperative_groups.h>
 
 #include "mlp_common.cuh"
+#include "rk_control.cuh"
+#include "rk_tableau.h"
 
 namespace cg = cooperative_groups;
 
@@ -43,20 +45,9 @@ namespace cfm {
 
 namespace {
 
-__constant__ float oC[7] = {0.f, 1.f / 5, 3.f / 10, 4.f / 5, 8.f / 9, 1.f, 1.f};
-__constant__ float oA[7][6] = {
-    {0, 0, 0, 0, 0, 0},
-    {1.f / 5, 0, 0, 0, 0, 0},
-    {3.f / 40, 9.f / 40, 0, 0, 0, 0},
-    {44.f / 45, -56.f / 15, 32.f / 9, 0, 0, 0},
-    {19372.f / 6561, -25360.f / 2187, 64448.f / 6561, -212.f / 729, 0, 0},
-    {9017.f / 3168, -355.f / 33, 46732.f / 5247, 49.f / 176, -5103.f / 18656, 0},
-    {35.f / 384, 0.f, 500.f / 1113, 125.f / 192, -2187.f / 6784, 11.f / 84}};
-__constant__ float oE[7] = {(float)(35.0 / 384 - 1951.0 / 21600), 0.f,
-                            (float)(500.0 / 1113 - 22642.0 / 50085),
-                            (float)(125.0 / 192 - 451.0 / 720),
-                            (float)(-2187.0 / 6784 + 12231.0 / 42400),
-                            (float)(11.0 / 84 - 649.0 / 6300), (float)(-1.0 / 60)};
+__constant__ float kC[7] = CFM_RK_C_INIT;
+__constant__ float kA[7][6] = CFM_RK_A_INIT;
+__constant__ float kE[7] = CFM_RK_E_INIT;
 
 struct OdeSmallParams {
   const float *W0, *b0, *W1, *b1, *W2, *b2, *W3, *b3;  // torch Linear layout [out][in]
@@ -446,34 +437,28 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
     return;
   }
 
-  // ---- dopri5 (torchdyn _adaptive_odeint semantics; scalar controller replicated in every thread) ----
-  const float atol = p.atol, rtol = p.rtol;
-  float t = __ldg(p.t_span), dt = 0.f, dt_old = 0.f, ratio = 0.f;
-  const float t_end = __ldg(p.t_span + n_span - 1);
-  int ckpt = 1, ckpt_flag = 0, done = 0, accepted = 0, rejected = 0, nfe = 0, pbuf = 0;
-
-  auto prestep = [&]() {
-    if (!(t < t_end)) { done = 1; return; }
-    if (t + dt > t_end) dt = t_end - t;
-    if (ckpt < n_span && t + dt > __ldg(p.t_span + ckpt)) {
-      dt_old = dt;
-      ckpt_flag = 1;
-      dt = __ldg(p.t_span + ckpt) - t;
-    }
-  };
+  // ---- dopri5 (torchdyn _adaptive_odeint semantics; rk_control.cuh's controller, replicated in every thread) ----
+  cfm_rk_state s = {};
+  s.atol = p.atol;
+  s.rtol = p.rtol;
+  s.t = __ldg(p.t_span);
+  s.t_end = __ldg(p.t_span + n_span - 1);
+  s.n_span = n_span;
+  int pbuf = 0;
 
   {
     // k1 = f(t0, x); Hairer's initial step: d0 = |x/sc|, d1 = |f0/sc|
     double s2[2] = {0.0, 0.0};
     for (int g = 0; g < rpw; g += RB) {
       if (row_of(g) >= B) break;
-      mlp_eval<U, CNF>(sm, pl, dim, tv, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 1), slot(g + 1, 1), lane);
+      mlp_eval<U, CNF>(sm, pl, dim, tv, act, slot(g, 0), slot(g + 1, 0), s.t, hA, hB, slot(g, 1), slot(g + 1, 1),
+                       lane);
 #pragma unroll
       for (int m = 0; m < RB; ++m) {
         if (row_of(g + m) >= B) continue;
         for (int e = lane; e < sw; e += 32) {
           const float xv = slot(g + m, 0)[e], f0 = slot(g + m, 1)[e];
-          const float sc = atol + fabsf(xv) * rtol;
+          const float sc = rk_init_scale(xv, s.atol, s.rtol);
           const float a = xv / sc, b = f0 / sc;
           s2[0] += (double)a * a;
           s2[1] += (double)b * b;
@@ -482,8 +467,7 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
     }
     grid_sum<2>(grid, s2, p.partials, pbuf, red);
     pbuf ^= 1;
-    const float d0 = (float)sqrt(s2[0] / numel), d1 = (float)sqrt(s2[1] / numel);
-    const float h0 = (d0 < 1e-5f || d1 < 1e-5f) ? 1e-6f : 0.01f * d0 / d1;
+    const float h0 = rk_h0(s2[0], s2[1], numel);
     double s1[1] = {0.0};
     for (int g = 0; g < rpw; g += RB) {
       if (row_of(g) >= B) break;
@@ -491,12 +475,12 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
       for (int m = 0; m < RB; ++m)
         for (int e = lane; e < sw; e += 32) xin[m * dimp + e] = fmaf(h0, slot(g + m, 1)[e], slot(g + m, 0)[e]);
       __syncwarp();
-      mlp_eval<U, CNF>(sm, pl, dim, tv, act, xin, xin + dimp, t + h0, hA, hB, slot(g, 2), slot(g + 1, 2), lane);
+      mlp_eval<U, CNF>(sm, pl, dim, tv, act, xin, xin + dimp, s.t + h0, hA, hB, slot(g, 2), slot(g + 1, 2), lane);
 #pragma unroll
       for (int m = 0; m < RB; ++m) {
         if (row_of(g + m) >= B) continue;
         for (int e = lane; e < sw; e += 32) {
-          const float sc = atol + fabsf(slot(g + m, 0)[e]) * rtol;
+          const float sc = rk_init_scale(slot(g + m, 0)[e], s.atol, s.rtol);
           const float q = (slot(g + m, 2)[e] - slot(g + m, 1)[e]) / sc;
           s1[0] += (double)q * q;
         }
@@ -504,18 +488,11 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
     }
     grid_sum<1>(grid, s1, p.partials, pbuf, red);
     pbuf ^= 1;
-    const float d2 = (float)sqrt(s1[0] / numel) / h0;
-    float h1;
-    if (d1 <= 1e-15f && d2 <= 1e-15f) h1 = fmaxf(1e-6f, h0 * 1e-3f);
-    else h1 = powf(0.01f / fmaxf(d1, d2), 1.f / 6.f);
-    dt = fminf(100.f * h0, h1);
-    dt_old = h0;
-    nfe = 2;
-    prestep();
+    rk_init_step(s, h0, s2[1], s1[0], numel, p.t_span);
   }
 
   int steps = 0;
-  while (!done && steps < p.max_steps) {
+  while (!s.done && steps < p.max_steps) {
     ++steps;
     double es[1] = {0.0};
     for (int g = 0; g < rpw; g += RB) {
@@ -524,7 +501,7 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
       for (int stage = 1; stage <= 6; ++stage) {
         float a[6];
 #pragma unroll
-        for (int q = 0; q < 6; ++q) a[q] = dt * oA[stage][q];
+        for (int q = 0; q < 6; ++q) a[q] = s.dt * kA[stage][q];
         float* d0p = stage < 6 ? xin : slot(g, 8);
         float* d1p = stage < 6 ? xin + dimp : slot(g + 1, 8);
 #pragma unroll
@@ -535,12 +512,12 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
             float v = x[e];
 #pragma unroll
             for (int q = 0; q < 6; ++q)
-              if (q < stage && oA[stage][q] != 0.f) v = fmaf(a[q], slot(g + m, 1 + q)[e], v);
+              if (q < stage && kA[stage][q] != 0.f) v = fmaf(a[q], slot(g + m, 1 + q)[e], v);
             dst[e] = v;
           }
         }
         __syncwarp();
-        mlp_eval<U, CNF>(sm, pl, dim, tv, act, d0p, d1p, t + oC[stage] * dt, hA, hB, slot(g, 1 + stage),
+        mlp_eval<U, CNF>(sm, pl, dim, tv, act, d0p, d1p, s.t + kC[stage] * s.dt, hA, hB, slot(g, 1 + stage),
                     slot(g + 1, 1 + stage), lane);
       }
 #pragma unroll
@@ -551,44 +528,16 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
           float er = 0.f;
 #pragma unroll
           for (int q = 0; q < 7; ++q)
-            if (oE[q] != 0.f) er = fmaf(oE[q], slot(g + m, 1 + q)[e], er);
-          er *= dt;
-          const float tol = atol + rtol * fmaxf(fabsf(x[e]), fabsf(slot(g + m, 8)[e]));
-          const float rr = er / tol;
+            if (kE[q] != 0.f) er = fmaf(kE[q], slot(g + m, 1 + q)[e], er);
+          er *= s.dt;
+          const float rr = er / rk_err_tol(x[e], slot(g + m, 8)[e], s.atol, s.rtol);
           es[0] += (double)rr * (double)rr;
         }
       }
     }
     grid_sum<1>(grid, es, p.partials, pbuf, red);
     pbuf ^= 1;
-    // ---- controller (rk.cu rk_control_kernel, torchdyn order) ----
-    ratio = (float)sqrt(es[0] / numel);
-    nfe += 6;
-    const bool accept = ratio <= 1.f;
-    int save_slot = -1;
-    if (accept) {
-      float tn = t + dt;
-      if (ckpt < n_span && (tn == __ldg(p.t_span + ckpt) || ckpt_flag)) {
-        tn = __ldg(p.t_span + ckpt);
-        save_slot = ckpt;
-        ckpt++;
-      }
-      t = tn;
-      accepted++;
-    } else {
-      rejected++;
-    }
-    float ndt = dt;
-    if (ckpt_flag) { ndt = dt_old - dt; ckpt_flag = 0; }
-    if (ratio == 0.f) {
-      ndt = ndt * 10.f;
-    } else {
-      const float min_factor = ratio < 1.f ? 1.f : 0.2f;
-      const float factor = fminf(10.f, fmaxf(0.9f / powf(ratio, 0.2f), min_factor));
-      ndt = ndt * factor;
-    }
-    dt = ndt;
-    prestep();
+    const bool accept = rk_control(s, (float)sqrt(es[0] / numel), p.t_span);
     // ---- commit: x <- xnew, k1 <- k7 (FSAL), checkpoint ----
     if (accept) {
       for (int j = 0; j < rpw; ++j) {
@@ -598,18 +547,15 @@ __global__ void __launch_bounds__(MAXT, 1) ode_small_kernel(const OdeSmallParams
           const float v = slot(j, 8)[e];
           slot(j, 0)[e] = v;
           slot(j, 1)[e] = slot(j, 7)[e];
-          if (save_slot >= 0) p.traj[((int64_t)save_slot * B + r) * sw + e] = v;
+          if (s.save_slot >= 0) p.traj[((int64_t)s.save_slot * B + r) * sw + e] = v;
         }
       }
       __syncwarp();
     }
   }
   if (blockIdx.x == 0 && tid == 0) {
-    cfm_rk_state* st = p.st;
-    st->t = t; st->dt = dt; st->t_end = t_end; st->atol = atol; st->rtol = rtol;
-    st->dt_old = dt_old; st->ratio = ratio; st->ckpt_flag = ckpt_flag; st->ckpt = ckpt;
-    st->n_span = n_span; st->commit = 0; st->done = done; st->save_slot = -1;
-    st->accepted = accepted; st->rejected = rejected; st->nfe = nfe; st->err_acc = 0.0;
+    s.save_slot = -1;  // every checkpoint is already in traj
+    *p.st = s;
   }
 }
 

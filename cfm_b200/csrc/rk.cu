@@ -6,7 +6,7 @@
 // controller is a handful of scalars.  They live in a device struct (cfm_rk_state): every kernel
 // of a step reads t/dt from it, the error norm is accumulated into it, and a one-thread control
 // kernel does accept/reject, checkpoint clipping and step-size adaptation in fp32 exactly in the
-// order torchdyn's _adaptive_odeint does.  A full step (6 stage-input kernels + 6 MLP forwards +
+// order torchdyn's _adaptive_odeint does (rk_control.cuh, shared with ode_small.cu).  A full step (6 stage-input kernels + 6 MLP forwards +
 // error norm + control + commit) is therefore enqueued without any host round trip.
 //
 // Buffers (fp32, numel = B*D each): x, xnew, xs (stage input), k[0..6] contiguous (k1..k7).
@@ -14,6 +14,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "rk_control.cuh"
 #include "rk_tableau.h"
 
 namespace cfm {
@@ -172,60 +173,18 @@ __global__ void rk_error_norm_kernel(cfm_rk_state* st, const float* __restrict__
         if (kE[j] != 0.f) e = fmaf(kE[j], k[(int64_t)j * numel + i], e);
     }
     e *= dt;
-    const float tol = atol + rtol * fmaxf(fabsf(x[i]), fabsf(xnew[i]));
-    const float r = e / tol;
+    const float r = e / rk_err_tol(x[i], xnew[i], atol, rtol);
     acc += (double)r * (double)r;
   }
   const double t = block_sum_to(acc, red);
   if (threadIdx.x == 0) atomicAdd(&st->err_acc, t);
 }
 
-__device__ __forceinline__ void rk_prestep(cfm_rk_state* st, const float* t_span) {
-  // top of torchdyn's while-loop for the NEXT step: clip to T, clip to the next checkpoint
-  if (!(st->t < st->t_end)) { st->done = 1; return; }
-  if (st->t + st->dt > st->t_end) st->dt = st->t_end - st->t;
-  if (st->ckpt < st->n_span && st->t + st->dt > t_span[st->ckpt]) {
-    st->dt_old = st->dt;
-    st->ckpt_flag = 1;
-    st->dt = t_span[st->ckpt] - st->t;
-  }
-}
-
 __global__ void rk_control_kernel(cfm_rk_state* st, const float* __restrict__ t_span, int64_t numel) {
   if (st->done) { st->commit = 0; return; }  // a step enqueued past the end of the interval is a no-op
   const float ratio = (float)sqrt(st->err_acc / (double)numel);
-  st->ratio = ratio;
   st->err_acc = 0.0;
-  st->nfe += 6;
-  const bool accept = ratio <= 1.f;
-  st->save_slot = -1;
-  st->commit = accept ? 1 : 0;
-  if (accept) {
-    float tn = st->t + st->dt;
-    // torchdyn records a checkpoint when t + dt == t_span[ckpt]; a step that was clipped to land
-    // on the checkpoint is snapped onto it so fp32 rounding of t + (t_ckpt - t) cannot miss it
-    if (st->ckpt < st->n_span && (tn == t_span[st->ckpt] || st->ckpt_flag)) {
-      tn = t_span[st->ckpt];
-      st->save_slot = st->ckpt;
-      st->ckpt++;
-    }
-    st->t = tn;
-    st->accepted++;
-  } else {
-    st->rejected++;
-  }
-  float dt = st->dt;
-  if (st->ckpt_flag) { dt = st->dt_old - dt; st->ckpt_flag = 0; }
-  // adapt_step(dt, ratio, safety=.9, min_factor=.2, max_factor=10, order=5)
-  if (ratio == 0.f) {
-    dt = dt * 10.f;
-  } else {
-    const float min_factor = ratio < 1.f ? 1.f : 0.2f;
-    const float factor = fminf(10.f, fmaxf(0.9f / powf(ratio, 0.2f), min_factor));
-    dt = dt * factor;
-  }
-  st->dt = dt;
-  rk_prestep(st, t_span);
+  st->commit = rk_control(*st, ratio, t_span) ? 1 : 0;
 }
 
 // accepted: x <- xnew, k1 <- k7 (FSAL), optional checkpoint copy
@@ -266,7 +225,7 @@ __global__ void rk_init_reduce_a(const cfm_rk_state* __restrict__ st, const floa
     float s0 = 0.f, s1 = 0.f;  // four squares per partial: fp32 is ample, the long sums are float64
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      const float sc = atol + fabsf(xs[c]) * rtol;
+      const float sc = rk_init_scale(xs[c], atol, rtol);
       const float p = xs[c] / sc, q = fs[c] / sc;
       s0 = fmaf(p, p, s0);
       s1 = fmaf(q, q, s1);
@@ -275,7 +234,7 @@ __global__ void rk_init_reduce_a(const cfm_rk_state* __restrict__ st, const floa
     a1 += (double)s1;
   }
   for (int64_t i = (n4 << 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < numel; i += stride) {
-    const float sc = atol + fabsf(x[i]) * rtol;
+    const float sc = rk_init_scale(x[i], atol, rtol);
     const float p = x[i] / sc, q = f0[i] / sc;
     a0 += (double)p * p;
     a1 += (double)q * q;
@@ -286,19 +245,11 @@ __global__ void rk_init_reduce_a(const cfm_rk_state* __restrict__ st, const floa
   t = block_sum_to(a1, red);
   if (threadIdx.x == 0) atomicAdd(&scratch[1], t);
 }
-__device__ __forceinline__ float rk_h0(const double* scratch, int64_t numel) {
-  const float d0 = (float)sqrt(scratch[0] / (double)numel);
-  const float d1 = (float)sqrt(scratch[1] / (double)numel);
-  return (d0 < 1e-5f || d1 < 1e-5f) ? 1e-6f : 0.01f * d0 / d1;
-}
-__global__ void rk_init_probe(cfm_rk_state* st, const float* __restrict__ x, const float* __restrict__ f0,
+__global__ void rk_init_probe(const cfm_rk_state* st, const float* __restrict__ x, const float* __restrict__ f0,
                               float* __restrict__ x_probe, float* __restrict__ t_stage,
                               const double* __restrict__ scratch, int64_t numel, int64_t numel_global) {
-  const float h0 = rk_h0(scratch, numel_global);
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    st->dt_old = h0;
-    if (t_stage) *t_stage = st->t + h0;
-  }
+  const float h0 = rk_h0(scratch[0], scratch[1], (double)numel_global);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && t_stage) *t_stage = st->t + h0;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < numel; i += stride)
     x_probe[i] = fmaf(h0, f0[i], x[i]);
@@ -311,7 +262,7 @@ __global__ void rk_init_reduce_b(const cfm_rk_state* __restrict__ st, const floa
   double a = 0.0;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < numel; i += stride) {
-    const float sc = atol + fabsf(x[i]) * rtol;
+    const float sc = rk_init_scale(x[i], atol, rtol);
     const float q = (f1[i] - f0[i]) / sc;
     a += (double)q * q;
   }
@@ -320,18 +271,8 @@ __global__ void rk_init_reduce_b(const cfm_rk_state* __restrict__ st, const floa
 }
 __global__ void rk_init_finish(cfm_rk_state* st, const float* __restrict__ t_span,
                                const double* __restrict__ scratch, int64_t numel) {
-  const float h0 = rk_h0(scratch, numel);
-  const float d1 = (float)sqrt(scratch[1] / (double)numel);
-  const float d2 = (float)sqrt(scratch[2] / (double)numel) / h0;
-  float h1;
-  if (d1 <= 1e-15f && d2 <= 1e-15f) h1 = fmaxf(1e-6f, h0 * 1e-3f);
-  else h1 = powf(0.01f / fmaxf(d1, d2), 1.f / 6.f);
-  st->dt = fminf(100.f * h0, h1);
-  st->nfe += 2;
-  st->ckpt = 1;
-  st->ckpt_flag = 0;
-  st->done = 0;
-  rk_prestep(st, t_span);
+  const double n = (double)numel;
+  rk_init_step(*st, rk_h0(scratch[0], scratch[1], n), scratch[1], scratch[2], n, t_span);
 }
 
 __global__ void axpy_kernel(const float* __restrict__ x, const float* __restrict__ k, float h,

@@ -1,5 +1,5 @@
-// Dormand-Prince 5(4) coefficients, one definition for rk.cu (device constants) and for the host code that hands
-// a stage's row to the fused MLP kernel (mlp_h3.cu).  torchdyn's DormandPrince45 tableau (un-vendored dependency,
+// Dormand-Prince 5(4) coefficients, one definition for both ODE drivers: rk.cu (device constants and compile-time
+// stage rows) and ode_small.cu (device constants).  torchdyn's DormandPrince45 tableau (un-vendored dependency,
 // SURVEY.md Appendix B), pinned against SciPy's RK45 in tests/test_oracle.py.
 #pragma once
 

@@ -57,6 +57,12 @@ def _decreasing(t_span):
     return t_span.numel() >= 2 and bool(t_span[1] < t_span[0])
 
 
+def _rk_stats(cur, **extra):
+    """``NeuralODE.stats`` from the controller state (``_ffi.RkState``) a device run left."""
+    return {"nfe": cur.nfe, "accepted": cur.accepted, "rejected": cur.rejected, "t": cur.t,
+            "last_ratio": cur.ratio, **extra}
+
+
 class NeuralODE(torch.nn.Module):
     """Subset of torchdyn.core.NeuralODE used by the reference examples."""
 
@@ -95,20 +101,21 @@ class NeuralODE(torch.nn.Module):
         if not x.is_cuda:
             raise _ffi.CfmLibraryError("NeuralODE.trajectory needs CUDA inputs (no CPU fallback)")
         dev = x.device
+        t_span = torch.as_tensor(t_span, dtype=torch.float32)
+        reverse = self.solver == "dopri5" and _decreasing(t_span)  # see the module docstring
         with torch.cuda.device(dev):  # the library launches on the CURRENT device: make it the tensors' one
-            if cnf:
-                return self._cnf_trajectory_on(mlp, x, t_span, dev)
-            return self._trajectory_on(mlp, x, t_span, dev)
+            if reverse:
+                mlp, t_span = mlp._time_reversed(), -t_span
+            out = (self._cnf_trajectory_on if cnf else self._trajectory_on)(mlp, x, t_span, dev)
+        if reverse:
+            self.stats["t"] = -self.stats["t"]
+        return out
 
     def _trajectory_on(self, mlp, x, t_span, dev):
         shape = x.shape
         x0 = x.detach().reshape(shape[0], -1).float().contiguous()
-        t_span = torch.as_tensor(t_span, dtype=torch.float32)
         if self.lockstep is not None and self.solver != "dopri5":
             raise NotImplementedError("lock-step sharding applies to the adaptive solver (dopri5)")
-        reverse = self.solver == "dopri5" and _decreasing(t_span)
-        if reverse:
-            mlp, t_span = mlp._time_reversed(), -t_span
         if self.lockstep is None and self.use_fused_small and t_span.numel() >= 2 \
                 and _ffi.lib().cfm_ode_small_supported(x0.shape[0], x0.shape[1], mlp.w, mlp.out_dim):
             out = self._fused_small(mlp, x0, t_span.to(dev).contiguous())
@@ -118,8 +125,6 @@ class NeuralODE(torch.nn.Module):
             # the span stays on the host (where callers build it): the plan keeps a device copy and refreshes it only
             # when the values change, so a repeated call neither uploads nor reads back anything before the first kernel
             out = self._dopri5(mlp, x0, t_span.detach().cpu().contiguous())
-        if reverse:
-            self.stats["t"] = -self.stats["t"]
         return out.reshape(out.shape[0], *shape)
 
     def _cnf_trajectory_on(self, mlp, x, t_span, dev):
@@ -130,7 +135,6 @@ class NeuralODE(torch.nn.Module):
         if x.dim() != 2 or x.shape[1] != mlp.dim + 1:
             raise ValueError(f"cnf_wrapper: expected a state of shape (B, {mlp.dim + 1}) (x and the log-density "
                              f"column), got {tuple(x.shape)}")
-        t_span = torch.as_tensor(t_span, dtype=torch.float32)
         if t_span.numel() < 2:
             raise ValueError("cnf_wrapper: t_span needs at least two points")
         if mlp.out_dim != mlp.dim or not _ffi.lib().cfm_ode_small_cnf_supported(x.shape[0], mlp.dim, mlp.w):
@@ -138,13 +142,7 @@ class NeuralODE(torch.nn.Module):
                 f"cnf_wrapper: no exact-likelihood kernel for B={x.shape[0]}, dim={mlp.dim}, w={mlp.w}, "
                 f"out_dim={mlp.out_dim} (it takes w in {{32, 64, 128}}, dim <= 8, out_dim == dim and batches whose "
                 "state fits in shared memory)")
-        reverse = self.solver == "dopri5" and _decreasing(t_span)
-        if reverse:
-            mlp, t_span = mlp._time_reversed(), -t_span
-        out = self._fused_small(mlp, x.detach().float().contiguous(), t_span.to(dev).contiguous(), cnf=True)
-        if reverse:
-            self.stats["t"] = -self.stats["t"]
-        return out
+        return self._fused_small(mlp, x.detach().float().contiguous(), t_span.to(dev).contiguous(), cnf=True)
 
     # ------------------------------------------------------------------------------------
     def _fused_small(self, mlp, x0, t_span, cnf=False):
@@ -173,8 +171,7 @@ class NeuralODE(torch.nn.Module):
         cur = _ffi.RkState.from_buffer_copy(bytes(st.cpu().numpy().tobytes()))
         if not cur.done:
             raise RuntimeError("dopri5: step budget exhausted")
-        self.stats = {"nfe": cur.nfe, "accepted": cur.accepted, "rejected": cur.rejected, "t": cur.t,
-                      "last_ratio": cur.ratio, "graph": False, "fused": True}
+        self.stats = _rk_stats(cur, graph=False, fused=True)
         return traj
 
     def _euler(self, mlp, x, t_span):
@@ -358,9 +355,7 @@ class NeuralODE(torch.nn.Module):
         else:
             raise RuntimeError("dopri5: step budget exhausted")
         P["last_steps"] = int(cur.accepted) + int(cur.rejected)
-        self.stats = {"nfe": cur.nfe, "accepted": cur.accepted, "rejected": cur.rejected,
-                      "t": cur.t, "last_ratio": cur.ratio, "graph": P["graph"] is not None and not lock,
-                      "lockstep": lock}
+        self.stats = _rk_stats(cur, graph=P["graph"] is not None and not lock, lockstep=lock)
         return traj.clone()
 
 

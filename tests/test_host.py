@@ -309,8 +309,8 @@ def _eval_c_fraction_table(text):
 
 
 def test_rk_tableau_header_is_the_oracles_dormand_prince_tableau():
-    """csrc/rk_tableau.h feeds rk.cu's device constants and its compile-time stage rows: every coefficient equals the
-    oracle's (SciPy-pinned) Dormand-Prince tableau rounded to fp32."""
+    """csrc/rk_tableau.h feeds the device constants of both ODE drivers (rk.cu, with its compile-time stage rows, and
+    ode_small.cu): every coefficient equals the oracle's (SciPy-pinned) Dormand-Prince tableau rounded to fp32."""
     import re
     from oracle import vector_field as vf
     src = open(os.path.join(ROOT, "cfm_b200", "csrc", "rk_tableau.h")).read()
@@ -328,6 +328,27 @@ def test_rk_tableau_header_is_the_oracles_dormand_prince_tableau():
         # the header writes e.g. 44.f / 45: an fp32 quotient of exactly representable integers == fp32(44 / 45)
         assert [f32(v) for v in a[s]] == [f32(v) for v in row], s
     assert [f32(v) for v in e] == [f32(v) for v in vf._BERR]
+
+
+def test_both_ode_drivers_take_the_tableau_and_the_step_controller_from_one_place():
+    """The multi-kernel driver (rk.cu) and the one-launch kernel (ode_small.cu) must take the same dopri5 steps, so
+    the tableau lives only in rk_tableau.h (checked above against the oracle) and torchdyn's controller only in
+    rk_control.cuh.  A second copy would let one driver drift from the other unnoticed."""
+    import re
+    csrc = os.path.join(ROOT, "cfm_b200", "csrc")
+    # numerators of the Dormand-Prince a and b5 - b4 rows that no other formula here needs
+    coeff = re.compile(r"\b(19372|25360|64448|9017|46732|5103|22642|12231|1951)\b")
+    adapt = re.compile(r"powf\(\s*ratio\s*,\s*0\.2f\s*\)")  # adapt_step's ratio^(1/5)
+    for name in sorted(os.listdir(csrc)):
+        src = open(os.path.join(csrc, name)).read()
+        if name != "rk_tableau.h":
+            assert not coeff.search(src), f"{name} spells out Dormand-Prince coefficients; include rk_tableau.h"
+        if name != "rk_control.cuh":
+            assert not adapt.search(src), f"{name} restates the step controller; use rk_control.cuh"
+    for name in ("rk.cu", "ode_small.cu"):
+        src = open(os.path.join(csrc, name)).read()
+        for header in ("rk_tableau.h", "rk_control.cuh"):
+            assert re.search(r'^#include "' + re.escape(header) + '"', src, re.M), (name, header)
 
 
 def test_seeded_screening_bound_holds_on_sinkhorn_iterates():
