@@ -593,8 +593,8 @@ int plan_launch(int64_t B, int dim, bool cnf, Launch* out) {
       return 1;
     }
     // CNF: the tangent buffers grow with the warps per CTA while the per-CTA row state does not, so fewer warps
-    // with more row groups each may still fit
-    if (!cnf || nwarps == 4) return 0;
+    // with more row groups each may still fit -- down to one warp, which w = 128 with dim 7 or 8 needs at any batch
+    if (!cnf || nwarps == 1) return 0;
     nwarps /= 2;
     shape(nwarps);
   }
@@ -621,11 +621,17 @@ int launch_t(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {
   note_launches(1);
   return CFM_OK;
 }
+// No 1024-thread instantiation for w = 128: at 32 warps W1, W2 (128 KB) and the hidden buffers (64 KB) plus the row
+// state exceed the planner's 200 KB, so plan_launch never returns such a launch.
 template <int U>
 int launch(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {
   if (L.nwarps <= 8) return launch_t<U, 256, false>(p, L, s);
   if (L.nwarps <= 16) return launch_t<U, 512, false>(p, L, s);
-  return launch_t<U, 1024, false>(p, L, s);
+  if constexpr (U < 4) {
+    return launch_t<U, 1024, false>(p, L, s);
+  } else {
+    CFM_REQUIRE(false, "ode_small: %d warps per CTA at w = 128 (the planner gives at most 16)", L.nwarps);
+  }
 }
 template <int U>
 int launch_cnf(const OdeSmallParams& p, const Launch& L, cudaStream_t s) {

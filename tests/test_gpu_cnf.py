@@ -8,6 +8,7 @@ import torch
 
 import cnf_oracle as co
 from oracle import vector_field as vf
+from test_gpu_small_fields import assert_cnf_close, smooth_rows
 
 import cfm_b200
 from cfm_b200 import _ffi
@@ -137,22 +138,34 @@ def test_tutorial_log_likelihood_matches_stock_pytorch(act):
 
 
 def test_density_grid_40000_points_in_one_launch():
-    m, _ = _pair(seed=11)
+    m, mc = _pair(seed=11)
     g = torch.linspace(-3, 3, 200)
     xx, yy = torch.meshgrid(g, g, indexing="ij")
-    z = _state(torch.stack([xx.reshape(-1), yy.reshape(-1)], 1)).to(DEV)
+    zc = _state(torch.stack([xx.reshape(-1), yy.reshape(-1)], 1))
+    z = zc.to(DEV)
     assert _ffi.lib().cfm_ode_small_cnf_supported(40000, 2, 64)
     node = cfm_b200.NeuralODE(cfm_b200.cnf_wrapper(m), solver="euler")
     before = _ffi.lib().cfm_launch_count()
-    traj = node.trajectory(z, torch.linspace(1, 0, 201))
+    span = torch.linspace(1, 0, 201)
+    traj = node.trajectory(z, span)
     assert _ffi.lib().cfm_launch_count() - before == 1
     assert node.stats["fused"] and traj.shape == (201, 40000, 3) and torch.isfinite(traj).all()
-    # Euler rows are independent: a sub-batch integrates to the same bits
-    sub = node.trajectory(z[:333], torch.linspace(1, 0, 201))
+    # Euler rows are independent: a sub-batch integrates to the same bits, and sampled rows match the float64 oracle
+    sub = node.trajectory(z[:333], span)
     assert torch.equal(sub, traj[:, :333])
+    rows = torch.randperm(40000, generator=torch.Generator().manual_seed(13))[:1000]
+    ref = co.euler_any_direction(co.cnf_field(mc), zc[rows].double(), span.double())
+    assert (traj[:, rows.to(DEV)].cpu().double() - ref).abs().max() <= 1e-4 * max(1.0, ref.abs().max().item())
+    # dopri5: the log-density column is gated away from SELU's kink, where fp32 need not take float64's branch of act'
     node5 = cfm_b200.NeuralODE(cfm_b200.cnf_wrapper(m), solver="dopri5", atol=1e-4, rtol=1e-4)
     out = node5.trajectory(z, torch.linspace(1, 0, 2))
     assert node5.stats["fused"] and torch.isfinite(out).all()
+    seen = []
+    ref5, st = co.dopri5_any_direction(co.recording(co.cnf_field(mc), seen), zc.double(),
+                                       torch.linspace(1, 0, 2, dtype=torch.float64), 1e-4, 1e-4)
+    assert (node5.stats["nfe"], node5.stats["accepted"], node5.stats["rejected"]) == \
+        (st["nfe"], st["accepted"], st["rejected"])
+    assert_cnf_close(out.cpu().double(), ref5, smooth_rows(mc, seen, "selu"), 1e-4)
 
 
 def test_refusals():
