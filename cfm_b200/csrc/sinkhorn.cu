@@ -999,8 +999,10 @@ __global__ void plan_materialize_kernel(const float* __restrict__ M, int n0, int
   if (bad) atomicOr(status, CFM_FLAG_NONFINITE);
 }
 
+size_t sinkhorn_v2_compact_pitch(int n0, int n1);  // sinkhorn_v2.cu
+
 struct SkLayout {
-  size_t u, v0, v1, pm, ps, ring, total;
+  size_t u, v0, v1, pm, ps, ring, mq, mq_bytes, total;
 };
 static SkLayout sk_layout(int n0, int n1, int grid) {
   const size_t n1p = (size_t)(n1 + 3) / 4 * 4;
@@ -1012,6 +1014,8 @@ static SkLayout sk_layout(int n0, int n1, int grid) {
   L.pm = o; o += align_up((size_t)grid * n1p * 8, 256);
   L.ps = o; o += align_up((size_t)grid * n1p * 8, 256);
   L.ring = o; o += 8192;  // err ring (4 doubles) + per-CTA minima of the potential changes (2 x 512 floats)
+  L.mq_bytes = (size_t)n0 * sinkhorn_v2_compact_pitch(n0, n1);  // 3-byte cost copy (shapes whose fp32 M streams)
+  L.mq = o; o += align_up(L.mq_bytes, 256);
   L.total = o;
   return L;
 }
@@ -1080,6 +1084,7 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
     char* w = reinterpret_cast<char*>(workspace);
     p.u_work = w + L.u; p.v_work[0] = w + L.v0; p.v_work[1] = w + L.v1;
     p.part_m = w + L.pm; p.part_s = w + L.ps; p.err_ring = reinterpret_cast<double*>(w + L.ring);
+    p.mq = L.mq_bytes ? reinterpret_cast<unsigned char*>(w + L.mq) : nullptr;
   }
   // precise: -1 auto, 0 fp32, 1 float64, 2 fp32 on the generic kernel, 3 float64 with fp32 exponentials ("mixed"),
   // 4 = 3 without the screening of negligible terms

@@ -41,6 +41,8 @@ struct SkParams {
   int vec;          // float4 path usable
   int v_in_smem;
   float l2_resident_frac;  // sinkhorn_v2: share of each slab loaded with L2 evict_last (0: default policy)
+  unsigned char* mq;  // sinkhorn_v2: 3-byte fixed-point copy of M (n0 rows of ldc bytes; null: fp32 sweeps only)
+  int64_t ldc;        //              its row pitch in bytes, align16(3 * n1)
   int run_if;       // 0 always; 1 only when auto-mode resolves to fast; 2 only when it resolves to precise
   int timeline;     // seeded solver: globaltimer marks of one iteration (CFM_SK_TL; debug aid)
   int screen;       // mixed mode: fp32 screening of negligible terms (0 only for precise = 4, the unscreened reference)

@@ -21,9 +21,18 @@
 //     element per iteration instead of ~11 and two, and the smem stage is released as soon as it
 //     has been read.  Ranges are safe by construction: LSE is 1-Lipschitz, so the spreads of u and
 //     v are <= span and every product stays within 2^(+-3*span) << 2^127.
+//   * 3-BYTE COST STREAM (factored path, when fp32 M does not fit in the L2; status[3] = 4): the factored
+//     sweep only uses M through the exponent e = M*c2 - kappa in [0, span], so after the prologue it reads a
+//     fixed-point copy of e instead of M: q = rint(e / a), a = fl32(span / (2^23 - 1)), 3 bytes per element
+//     (12-byte groups of 4 columns, rows of ldc = align16(3*n1) bytes in the workspace).  The prologue sweep
+//     still reads fp32 rows and writes the copy (float64 encode, once per solve); iterations decode with no
+//     conversion instruction: the bit pattern 0x4B000000 | q is the float 2^23 + q, so e' = fmaf(F, a, -2^23 a)
+//     = fl(q*a) exactly up to the final rounding.  |e' - e| <= a/2 + ulp = span * 2^-24 + ulp; 25% fewer bytes.
 //   * per-CTA column partials -> [cta][n1] workspace -> grid barrier -> sliced combine -> v_new,
 //     marginal error -> grid barrier (identical to sinkhorn.cu).
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "sinkhorn_common.cuh"
 
@@ -73,6 +82,19 @@ __device__ __forceinline__ uint64_t v2_policy_evict_first() {
 }
 template <int NT>
 __device__ __forceinline__ void v2_consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
+
+// 3-byte stream: e = m*c2 - kappa in float64 (exact: a 24 x 24-bit product), quantised with one rounding and
+// clamped to [0, 2^23 - 1] (at m = cost_max the fp32 kappa may put e a rounding below 0; NaN -> 0, but a NaN cost
+// has already made the prologue's column potential NaN, and that reaches every potential as on the fp32 path)
+__device__ __forceinline__ uint32_t v2_encode(float m, float c2, float kappa, double qinv) {
+  const double e = (double)m * (double)c2 - (double)kappa;
+  return (uint32_t)fmin(fmax(rint(e * qinv), 0.0), 8388607.0);
+}
+// e' = fl(q * qa) of the entry in the low 24 bits of w: the bit pattern 0x4B000000 | q is the float 2^23 + q (q < 2^23:
+// byte 2 of an entry has its top bit clear), so subtracting 2^23 is exact and no conversion instruction is needed
+__device__ __forceinline__ float v2_q_decode(uint32_t w, float qa) {
+  return (__uint_as_float(0x4B000000u | (w & 0xFFFFFFu)) - 8388608.f) * qa;
+}
 
 // Reduce R per-lane values over the warp with a shared shuffle tree: at the stage with offset
 // `off` lanes whose bit `off` is set keep the odd member of each pair, the others the even one, so
@@ -124,8 +146,12 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   float2* rowpart = reinterpret_cast<float2*>(stages + (size_t)S * stage_floats);  // [2][R][16]
   uint64_t* full = reinterpret_cast<uint64_t*>(rowpart + 2 * R * kV2Warps);
   __shared__ double red[kV2Warps];
+  __shared__ int cslice[2];  // this CTA's columns in the combine step (in smem: a register there would spill)
 
   if (tid == 0) {
+    const int cpc = (n1 + nblk - 1) / nblk;
+    cslice[0] = b * cpc;
+    cslice[1] = min(n1, b * cpc + cpc);
     for (int s = 0; s < S; ++s) v2_mbar_init(&full[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -141,6 +167,9 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   const float loga = -log2f((float)n0), logb = -log2f((float)n1);
   const float kappa = c2 * cmaxv;  // = min_ij M_ij*c2 (most negative exponent), so E = ex2(M*c2 - kappa) >= 1
   const bool fact = (p.cost_max != nullptr) && (-kappa <= 40.f);  // span in log2 units
+  // 3-byte stream of the factored exponent (every sweep after the prologue; row pitch p.ldc bytes).  Its quantum
+  // and pitch are formed where they are used: long-lived values cost registers in the combine step.
+  const bool compact = fact && p.mq != nullptr;
 
   const int base = n0 / nblk, rem = n0 % nblk;
   const int r_begin = b * base + min(b, rem);
@@ -165,18 +194,26 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   // L2 residency: the first `resident` chunks of every slab are loaded evict_last (they stay in the
   // L2 from sweep to sweep), the rest evict_first (pure streaming): only the streaming part
   // crosses HBM every iteration.  p.l2_resident_frac <= 0 leaves the default policy.
-  const int resident = p.l2_resident_frac > 0.f ? (int)(p.l2_resident_frac * (float)nchunks) : -1;
-  const uint64_t pol_last = v2_policy_evict_last(), pol_first = v2_policy_evict_first();
+  // The 3-byte stream keeps the same resident BYTES (more chunks of the smaller rows); its fp32 prologue is read
+  // once and streams entirely.
+  // (`resident` switches to the 3-byte stream's value when the producer switches format, see below)
+  int resident = p.l2_resident_frac <= 0.f ? -1 : compact ? 0 : (int)(p.l2_resident_frac * (float)nchunks);
   // thread 0: issue the bulk copies of the next chunk into its (free) stage
   auto issue_next = [&]() {
     const int r0 = r_begin + p_chunk * R;
     const int rv = min(R, r_begin + nrows - r0);
-    v2_mbar_expect_tx(&full[p_st], (uint32_t)rv * (uint32_t)n1 * 4u);
+    const bool q = compact && issued >= nchunks;  // the first nchunks chunks are the prologue's
+    const uint32_t ldc = (uint32_t)p.ldc;
+    const uint32_t row_bytes = q ? ldc : (uint32_t)n1 * 4u;
+    const uint64_t pol = p_chunk < resident ? v2_policy_evict_last() : v2_policy_evict_first();
+    v2_mbar_expect_tx(&full[p_st], (uint32_t)rv * row_bytes);
     for (int r = 0; r < rv; ++r) {
-      float* dst = stages + (size_t)p_st * stage_floats + (size_t)r * n1p;
-      const float* src = p.M + (int64_t)(r0 + r) * p.ldm;
-      if (resident < 0) v2_bulk_load(dst, src, (uint32_t)n1 * 4u, &full[p_st]);
-      else v2_bulk_load_hint(dst, src, (uint32_t)n1 * 4u, &full[p_st], p_chunk < resident ? pol_last : pol_first);
+      unsigned char* dst = reinterpret_cast<unsigned char*>(stages + (size_t)p_st * stage_floats) +
+                           (size_t)r * (q ? ldc : (uint32_t)n1p * 4u);
+      const void* src = q ? static_cast<const void*>(p.mq + (int64_t)(r0 + r) * ldc)
+                          : static_cast<const void*>(p.M + (int64_t)(r0 + r) * p.ldm);
+      if (resident < 0) v2_bulk_load(dst, src, row_bytes, &full[p_st]);
+      else v2_bulk_load_hint(dst, src, row_bytes, &full[p_st], pol);
     }
     ++issued;
     p_chunk += p_dir;
@@ -184,8 +221,13 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
     else if (p_chunk < 0) { p_chunk = 0; p_dir = 1; }
     if (++p_st == S) p_st = 0;
   };
+  // The ring runs S chunks ahead across sweeps, and the prologue's last S chunks are iteration 0's first: their
+  // 3-byte rows are written after the point where the ring would issue their refills.  So no chunk of the 3-byte
+  // stream is issued before the whole slab is encoded and fenced (one ring fill per solve, issued right after the
+  // prologue); the copy is reused from call to call, and an early read would return the previous coupling's rows.
+  auto may_issue = [&]() { return issued < nchunks || consumed_total != 0 || !compact; };
   if (tid == 0)
-    for (int q = 0; q < S; ++q) issue_next();  // initial fill (wraps into the next sweep if S > nchunks)
+    for (int q = 0; q < S && may_issue(); ++q) issue_next();  // initial fill (wraps into the next sweep if S > nchunks)
 
   // ---- one fused sweep ----
   auto sweep = [&](bool do_row, bool do_col, const float* v_cur) {
@@ -211,38 +253,69 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
       }
       float uref = 0.f;
       bool have_uref = !do_row;  // prologue: u = 0 everywhere, U = 1
+      // stage format: 0 fp32 rows, 1 fp32 rows that are also encoded into the 3-byte copy, 2 the 3-byte copy
+      const int fmt = !compact ? 0 : sweep_no == 0 ? 1 : 2;
+      const uint32_t ldc = (uint32_t)p.ldc;
+      // quantum span / (2^23 - 1) (span = 0: q = 0, e' = 0 = e) and encode scale; float64 divisions cost every
+      // thread about as much as a small shape's sweep has to spare, so only the stream's sweeps form them
+      const float qa = fmt != 0 ? (float)((double)(-kappa) / 8388607.0) : 0.f;
+      const double qinv = fmt == 1 && qa > 0.f ? 1.0 / (double)qa : 0.0;
       for (int cc = 0; cc < nchunks; ++cc) {
         const int chunk = (sweep_no & 1) ? nchunks - 1 - cc : cc;
         const int r0 = r_begin + chunk * R;
         const int rv = min(R, r_begin + nrows - r0);
         const float* sbase = stages + (uint32_t)c_st * stage_floats + tcol;
+        const unsigned char* qbase = reinterpret_cast<const unsigned char*>(stages + (uint32_t)c_st * stage_floats) + 12 * tid;
         float2* rp = rowpart + (cc & 1) * R * kV2Warps;
         v2_mbar_wait(&full[c_st], c_par);
         float4 E[R][KG];
-        if (full_cols && rv == R) {  // common case: no predicates in the hot loop
+        // E of every owned group of the stage; ALL: every thread owns KG valid groups of R rows (no predicates)
+        auto form_E = [&](auto FMT, auto ALL) {
+          constexpr int kFmt = decltype(FMT)::value;
+          constexpr bool kAll = decltype(ALL)::value;
 #pragma unroll
           for (int r = 0; r < R; ++r)
 #pragma unroll
             for (int k = 0; k < KG; ++k) {
-              const float4 mv = *reinterpret_cast<const float4*>(sbase + r * n1p + kV2Consumers * 4 * k);
-              E[r][k] = make_float4(ex2f(fmaf(mv.x, c2, nkap)), ex2f(fmaf(mv.y, c2, nkap)),
-                                    ex2f(fmaf(mv.z, c2, nkap)), ex2f(fmaf(mv.w, c2, nkap)));
-            }
-        } else {
-#pragma unroll
-          for (int r = 0; r < R; ++r) {
-            const float* srow = sbase + r * n1p;
-#pragma unroll
-            for (int k = 0; k < KG; ++k) {
-              E[r][k] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (gvalid[k] && r < rv) {
-                const float4 mv = *reinterpret_cast<const float4*>(srow + kV2Consumers * 4 * k);
-                E[r][k] = make_float4(ex2f(fmaf(mv.x, c2, nkap)), ex2f(fmaf(mv.y, c2, nkap)),
-                                      ex2f(fmaf(mv.z, c2, nkap)), ex2f(fmaf(mv.w, c2, nkap)));
+              if (!kAll) E[r][k] = make_float4(0.f, 0.f, 0.f, 0.f);
+              if (kAll || (gvalid[k] && r < rv)) {
+                if constexpr (kFmt == 2) {
+                  // 12 bytes = 4 entries; three 4-byte smem loads at a stride of 3 words (no bank conflicts)
+                  const uint32_t* w = reinterpret_cast<const uint32_t*>(qbase + r * ldc + 12 * kV2Consumers * k);
+                  const uint32_t w0 = w[0], w1 = w[1], w2 = w[2];
+                  E[r][k] = make_float4(ex2f(v2_q_decode(w0, qa)),
+                                        ex2f(v2_q_decode(__funnelshift_r(w0, w1, 24), qa)),
+                                        ex2f(v2_q_decode(__funnelshift_r(w1, w2, 16), qa)),
+                                        ex2f(v2_q_decode(w2 >> 8, qa)));
+                } else {
+                  const float4 mv = *reinterpret_cast<const float4*>(sbase + r * n1p + kV2Consumers * 4 * k);
+                  E[r][k] = make_float4(ex2f(fmaf(mv.x, c2, nkap)), ex2f(fmaf(mv.y, c2, nkap)),
+                                        ex2f(fmaf(mv.z, c2, nkap)), ex2f(fmaf(mv.w, c2, nkap)));
+                }
               }
             }
-          }
+        };
+        if (fmt == 1) {
+          // prologue: write this stage's rows into the 3-byte copy (its own pass: E is not live yet)
+#pragma unroll 1
+          for (int r = 0; r < rv; ++r)
+#pragma unroll
+            for (int k = 0; k < KG; ++k)
+              if (gvalid[k]) {
+                const float4 mv = *reinterpret_cast<const float4*>(sbase + r * n1p + kV2Consumers * 4 * k);
+                const uint32_t q0 = v2_encode(mv.x, c2, kappa, qinv), q1 = v2_encode(mv.y, c2, kappa, qinv);
+                const uint32_t q2 = v2_encode(mv.z, c2, kappa, qinv), q3 = v2_encode(mv.w, c2, kappa, qinv);
+                uint32_t* dst = reinterpret_cast<uint32_t*>(p.mq + (int64_t)(r0 + r) * ldc + 12 * (tid + kV2Consumers * k));
+                dst[0] = q0 | (q1 << 24);
+                dst[1] = (q1 >> 8) | (q2 << 16);
+                dst[2] = (q2 >> 16) | (q3 << 8);
+              }
         }
+        using kT = std::true_type;
+        using kF = std::false_type;
+        const bool all = full_cols && rv == R;  // common case: no predicates in the hot loop
+        if (fmt == 2) { if (all) form_E(std::integral_constant<int, 2>{}, kT{}); else form_E(std::integral_constant<int, 2>{}, kF{}); }
+        else { if (all) form_E(std::integral_constant<int, 0>{}, kT{}); else form_E(std::integral_constant<int, 0>{}, kF{}); }
         if (++c_st == S) { c_st = 0; c_par ^= 1u; }
         if (do_row) {
           float sr[R];
@@ -262,7 +335,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
         // every warp has now copied its part of the stage into registers: after this barrier the
         // stage is free, so thread 0 refills it with the chunk S positions ahead
         v2_consumer_barrier<NT>();
-        if (tid == 0) issue_next();
+        if (tid == 0 && may_issue()) issue_next();
         float U[R];
         if (do_row) {
           // fold the 16 per-warp partials: lanes 0-15 take row r, lanes 16-31 row r+1 (one tree for two rows)
@@ -425,8 +498,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   // ---- combine a slice of columns over all CTAs' partials ----
   auto combine = [&](const float* v_cur, float* v_new, bool have_cur, double* err_slot) {
     double err_local = 0.0;
-    const int cpc = (n1 + nblk - 1) / nblk;
-    const int c_begin = b * cpc, c_end = min(n1, c_begin + cpc);
+    const int c_begin = cslice[0], c_end = cslice[1];
     const int sub = tid & 7;
     for (int j0 = c_begin; j0 < c_end; j0 += (kV2Consumers >> 3)) {  // NT/8 columns per pass
       const int j = j0 + (tid >> 3);
@@ -508,6 +580,17 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   bool converged = false;
   double err = 1.0, prev_check_err = -1.0;
   sweep(false, true, nullptr);
+  if (compact) {
+    // the 3-byte rows were written through the generic proxy; the bulk copies read them through the async
+    // proxy.  Each slab is written and read by its own CTA only, so a CTA barrier suffices.
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+    __syncthreads();
+    if (tid == 0) {
+      if (resident >= 0)
+        resident = min(nchunks, (int)(p.l2_resident_frac * (float)nchunks * (4.f * (float)n1) / (float)p.ldc));
+      while (issued < consumed_total + S) issue_next();
+    }
+  }
   grid.sync();
   combine(nullptr, v_work[0], false, nullptr);
   grid.sync();
@@ -551,7 +634,8 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
     p.status[0] = flags;
     p.status[1] = iters;
     p.status[2] = 0;
-    p.status[3] = fact ? 3 : 2;  // kernel variant: 3 = factored, 2 = log-domain
+    p.status[3] = compact ? 4 : fact ? 3 : 2;  // kernel variant: 4 = factored on the 3-byte stream, 3 = factored,
+                                               // 2 = log-domain
     *p.err_out = err;
   }
 }
@@ -578,18 +662,32 @@ static int v2_launch_t(SkParams& p, cudaStream_t s) {
   return CFM_OK;
 }
 
+// fp32 M streams from HBM when it takes more than 3/4 of the L2 (the potentials, the column partials and the ring
+// refills share the rest); a smaller M stays resident by itself
+static bool v2_streams(int n0, int n1) { return (size_t)n0 * n1 * 4 > l2_bytes() / 4 * 3; }
+
+// Row pitch of the 3-byte cost copy when a shape takes that stream, else 0: the shapes this kernel covers
+// (n1 a multiple of 4, at most 8192; the launch also needs 16-byte aligned fp32 rows) whose fp32 M streams.  An M
+// that stays in the L2 keeps the fp32 sweep.  The workspace size and the launch both decide through this.
+size_t sinkhorn_v2_compact_pitch(int n0, int n1) {
+  if ((n1 & 3) != 0 || n1 > 8192 || !v2_streams(n0, n1)) return 0;
+  return align_up((size_t)n1 * 3, 16);
+}
+
 // returns CFM_OK when launched, 1 when this shape is not covered (caller uses sinkhorn.cu), <0 on error
 int sinkhorn_v2_launch(SkParams& p, cudaStream_t s) {
   if (!p.vec || p.n1p > 8192 || p.n1p != p.n1) return 1;
-  // L2 policy, from the device's L2 size: M that takes at most 3/4 of the L2 (the potentials, the column partials and
-  // the ring refills share the rest) stays resident by itself and keeps the default policy; a larger M streams, and
-  // the part of it kept evict_last from sweep to sweep is kSkResidentShare of the L2 (CFM_SK_L2 overrides it with a
-  // fraction of each slab).  Solve ms on an H100 80GB HBM3 (50 MB L2, 700 W limit; scripts/sk_l2_sweep.py): C2
-  // (M = 268 MB) with 0 / 8 / 16 / 40 MB resident 9.61 / 9.33 / 9.36 / 9.45; a 4096 x 4096 shard (67 MB) with
-  // 0 / 4 / 10 / 20 MB resident 2.91 / 2.58 / 2.51 / 2.52 -- about 10 MB, a fifth of the L2, suits both
+  p.ldc = (int64_t)sinkhorn_v2_compact_pitch(p.n0, p.n1);
+  if (p.ldc == 0) p.mq = nullptr;  // (the caller points mq at the workspace region, sized by the same rule)
+  // L2 policy, from the device's L2 size: M that stays resident by itself (v2_streams) keeps the default policy; a
+  // larger M streams, and the part of it kept evict_last from sweep to sweep is kSkResidentShare of the L2 (CFM_SK_L2
+  // overrides it with a fraction of each slab; the kernel keeps the same bytes resident on the 3-byte stream).  Solve
+  // ms on an H100 80GB HBM3 (50 MB L2, 700 W limit; scripts/sk_l2_sweep.py), fp32 stream: C2 (M = 268 MB) with
+  // 0 / 8 / 16 / 40 MB resident 9.61 / 9.33 / 9.36 / 9.45; a 4096 x 4096 shard (67 MB) with 0 / 4 / 10 / 20 MB
+  // resident 2.91 / 2.58 / 2.51 / 2.52 -- about 10 MB, a fifth of the L2, suits both
   constexpr float kSkResidentShare = 0.2f;
   const size_t m_bytes = (size_t)p.n0 * p.n1 * 4, l2 = l2_bytes();
-  const bool streams = m_bytes > l2 / 4 * 3;
+  const bool streams = v2_streams(p.n0, p.n1);
   static float l2frac = -2.f;
   if (l2frac < -1.f) { const char* e = getenv("CFM_SK_L2"); l2frac = e ? (float)atof(e) : -1.f; }
   p.l2_resident_frac = !streams ? 0.f : l2frac >= 0.f ? l2frac : fminf(1.f, kSkResidentShare * (float)l2 / (float)m_bytes);
