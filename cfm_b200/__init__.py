@@ -15,8 +15,9 @@ from .conditional_flow_matching import (ConditionalFlowMatcher,  # noqa: F401
                                         SchrodingerBridgeConditionalFlowMatcher,
                                         TargetConditionalFlowMatcher,
                                         VariancePreservingConditionalFlowMatcher, pad_t_like_x)
-from .models import MLP, cnf_wrapper, torch_wrapper  # noqa: F401
+from .models import MLP, SDE, cnf_wrapper, torch_wrapper  # noqa: F401
 from .ode import NeuralODE  # noqa: F401
 from .optimal_transport import CouplingStream, OTPlanSampler, wasserstein  # noqa: F401
+from .sde import sdeint  # noqa: F401
 
 __version__ = "0.1.0"

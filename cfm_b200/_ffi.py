@@ -76,6 +76,9 @@ SIGNATURES = {
     "cfm_ode_small_cnf_supported": (_i, [_i64, _i, _i]),
     "cfm_ode_small_cnf_trajectory_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _i64, _p, _i, _f, _f, _i, _p, _p, _p, _sz,
                                                           _p]),
+    "cfm_sde_small_supported": (_i, [_i64, _i, _i]),
+    "cfm_sde_small_euler_f32": (_i, [_p, _p, _i, _i, _i, _f, _p, _i64, _p, _i, _p, _p, _p, _i, C.c_uint64, _p, _p,
+                                     _p]),
 }
 
 _lock = threading.Lock()

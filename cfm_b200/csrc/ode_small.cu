@@ -34,6 +34,7 @@
 // layer inputs (hbuf grows by 1 + dim).  The f part runs exactly the instructions of the plain variant, so the
 // x columns are bit-identical to it; the trace costs about dim more forwards per evaluation.
 #include <cooperative_groups.h>
+#include <curand_philox4x32_x.h>
 
 #include "mlp_common.cuh"
 #include "rk_control.cuh"
@@ -126,7 +127,9 @@ __device__ __forceinline__ float act_deriv_fast(float x, int act) {
 // tangents, and dim <= 8 (the layer-3 branch that ends in a warp reduction).
 // Deliberately NOT inlined and with rolled loops: the kernel runs 1-2 warps per scheduler, and
 // straight-line code of a few thousand instructions would not stay in the instruction cache.
-template <int U, bool CNF>
+// Copy: the SDE kernel calls its own instantiation (Copy = 1, same source).  With one instantiation shared between
+// both kernels ptxas compiled the ODE kernels' call sites differently; with two, their code is exactly what it was.
+template <int U, bool CNF, int Copy = 0>
 __device__ __noinline__ void mlp_eval(const float* __restrict__ sm, const SmemPlan& pl, int dim, int tv, int act,
                                       const float* xin0, const float* xin1, float t, float* hA, float* hB,
                                       float* out0, float* out1, int lane) {
@@ -670,6 +673,203 @@ int trajectory(bool cnf, const char* what, const float* W0, const float* b0, con
   return launch<4>(p, L, s);
 }
 
+// ==== Schrodinger-bridge SDE sampling: fixed-step Euler-Maruyama, dy = [drift(t, y) + score(t, y)] dt + sigma dW ====
+// Two MLPs (drift, score) of the same shape, evaluated by mlp_eval<U, false> one after the other from two weight sets
+// staged side by side in shared memory.  The step grid is the same scalar sequence in every thread and rows are
+// independent, so there is no grid barrier and the launch is an ordinary one.  Outputs are linear interpolations
+// between the states before and after the step that brackets them (torchsde's linear_interp); the host tabulates,
+// per step, which outputs it brackets and their two weights.
+
+struct SdeSmallParams {
+  const float *W0[2], *b0[2], *W1[2], *b1[2], *W2[2], *b2[2], *W3[2], *b3[2];  // [0] drift, [1] score; [out][in]
+  int dim, act;
+  float sigma;
+  const float* x0;
+  int64_t B;
+  const float* grid;       // [n_steps + 1] step times
+  int n_steps;
+  const int* out_begin;    // [n_steps + 1]: step n brackets outputs out_begin[n] .. out_begin[n + 1] - 1 (all >= 1)
+  const float* out_a;      // [n_out] weight of the state before the bracketing step
+  const float* out_b;      // [n_out] weight of the state after it
+  uint64_t seed;
+  const float* dw;         // nullable: [n_steps][B][dim] Brownian increments instead of the device stream
+  float* traj;             // [n_out][B][dim]
+  int rows_per_warp;
+};
+
+constexpr int kSdeSlots = 4;  // y, y before the last step, drift(t, y), score(t, y)
+
+struct SdePlan {
+  SmemPlan net;  // offsets of ONE weight set (net.dimp: padded row length); the score set starts `set2` floats later
+  size_t set2, hbuf, state, total;
+};
+__host__ __device__ inline SdePlan sde_small_plan(int dim, int w, int nwarps, int rpw) {
+  SdePlan s;
+  s.net = ode_small_plan(dim, w, 0, 0);  // with no warps nothing is laid out after b3: hbuf = one weight set's floats
+  s.set2 = s.net.hbuf;
+  size_t o = 2 * s.set2;
+  s.hbuf = o;
+  o += (size_t)nwarps * RB * 2 * w;
+  s.state = o;
+  o += (size_t)nwarps * rpw * kSdeSlots * s.net.dimp;
+  s.total = o * sizeof(float);
+  return s;
+}
+
+// Standard normal of (step n, row r, column c): one Philox4x32-10 block per 4 columns, 24-bit uniforms in (0, 1),
+// Box-Muller on (u0, u1) for columns 4q, 4q + 1 and on (u2, u3) for 4q + 2, 4q + 3.  Depends on nothing else.
+__device__ __forceinline__ float sde_normal(uint64_t seed, int n, int64_t r, int c) {
+  const uint4 x = curand_Philox4x32_10(
+      make_uint4((unsigned)(c >> 2), (unsigned)(uint64_t)r, (unsigned)((uint64_t)r >> 32), (unsigned)n),
+      make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  const bool hi = c & 2;
+  const unsigned xa = hi ? x.z : x.x, xb = hi ? x.w : x.y;
+  const float ua = __fmaf_rn((float)(xa >> 8), 0x1p-24f, 0x1p-25f);  // exact: 24-bit integer * 2^-24 + 2^-25
+  const float ub = __fmaf_rn((float)(xb >> 8), 0x1p-24f, 0x1p-25f);
+  float s, co;
+  sincospif(2.f * ub, &s, &co);
+  return sqrtf(-2.f * logf(ua)) * ((c & 1) ? s : co);
+}
+
+template <int U, int MAXT>
+__global__ void __launch_bounds__(MAXT, 1) sde_small_kernel(const SdeSmallParams p) {
+  constexpr int W = 32 * U;
+  extern __shared__ __align__(16) float sm[];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  const int dim = p.dim, act = p.act, rpw = p.rows_per_warp, in0 = dim + 1;
+  const SdePlan pl = sde_small_plan(dim, W, nwarps, rpw);
+  const SmemPlan& np = pl.net;
+  const int dimp = np.dimp;
+
+  // ---- stage both weight sets (transposed, as ode_small_kernel does); the time column is always present ----
+#pragma unroll 1
+  for (int q = 0; q < 2; ++q) {
+    float* ws = sm + q * pl.set2;
+    for (int idx = tid; idx < W * dim; idx += blockDim.x) {
+      const int u = idx / dim, i = idx % dim;
+      ws[np.wt0 + (size_t)i * W + u] = p.W0[q][(size_t)u * in0 + i];
+    }
+    for (int u = tid; u < W; u += blockDim.x) {
+      ws[np.wtime + u] = p.W0[q][(size_t)u * in0 + dim];
+      ws[np.b0 + u] = p.b0[q][u];
+      ws[np.b1 + u] = p.b1[q][u];
+      ws[np.b2 + u] = p.b2[q][u];
+    }
+    for (int idx = tid; idx < W * W; idx += blockDim.x) {
+      const int u = idx / W, i = idx % W;
+      ws[np.wt1 + (size_t)i * W + u] = p.W1[q][idx];
+      ws[np.wt2 + (size_t)i * W + u] = p.W2[q][idx];
+    }
+    for (int idx = tid; idx < dim * W; idx += blockDim.x) {
+      const int e = idx / W, i = idx % W;
+      ws[np.wt3 + (size_t)i * dim + e] = p.W3[q][idx];
+    }
+    for (int e = tid; e < dim; e += blockDim.x) ws[np.b3 + e] = p.b3[q][e];
+  }
+
+  float* hA = sm + pl.hbuf + (size_t)warp * 2 * RB * W;
+  float* hB = hA + RB * W;
+  const int64_t gwarp = (int64_t)blockIdx.x * nwarps + warp, wstride = (int64_t)gridDim.x * nwarps;
+  auto row_of = [&](int j) -> int64_t { return (gwarp + (int64_t)(j / RB) * wstride) * RB + (j % RB); };
+  auto slot = [&](int j, int s) -> float* {
+    return sm + pl.state + (((size_t)warp * rpw + j) * kSdeSlots + s) * dimp;
+  };
+  const int64_t B = p.B;
+
+  // ---- y0 -> state (rows past the batch: zeros, integrated along but never stored), traj[0] ----
+  for (int j = 0; j < rpw; ++j) {
+    const int64_t r = row_of(j);
+    for (int e = lane; e < dim; e += 32) {
+      const float v = r < B ? p.x0[r * dim + e] : 0.f;
+      slot(j, 0)[e] = v;
+      if (r < B) p.traj[r * dim + e] = v;
+    }
+  }
+  __syncthreads();
+
+  const float sigma = p.sigma;
+  for (int n = 0; n < p.n_steps; ++n) {
+    const float t = __ldg(p.grid + n), h = __ldg(p.grid + n + 1) - t;
+    const float sh = sqrtf(h);
+    const int k0 = __ldg(p.out_begin + n), k1 = __ldg(p.out_begin + n + 1);
+    for (int g = 0; g < rpw; g += RB) {
+      if (row_of(g) >= B) break;
+      mlp_eval<U, false, 1>(sm, np, dim, 1, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 2), slot(g + 1, 2),
+                            lane);
+      mlp_eval<U, false, 1>(sm + pl.set2, np, dim, 1, act, slot(g, 0), slot(g + 1, 0), t, hA, hB, slot(g, 3),
+                         slot(g + 1, 3), lane);
+#pragma unroll
+      for (int m = 0; m < RB; ++m) {
+        const int64_t r = row_of(g + m);
+        float* y = slot(g + m, 0);
+        float* yp = slot(g + m, 1);
+        const float* d = slot(g + m, 2);
+        const float* s = slot(g + m, 3);
+        for (int e = lane; e < dim; e += 32) {
+          float dW = 0.f;
+          if (r < B)
+            dW = p.dw ? __ldg(p.dw + ((int64_t)n * B + r) * dim + e) : __fmul_rn(sh, sde_normal(p.seed, n, r, e));
+          const float y0 = y[e];
+          const float y1 = __fadd_rn(fmaf(h, __fadd_rn(d[e], s[e]), y0), __fmul_rn(sigma, dW));
+          yp[e] = y0;
+          y[e] = y1;
+          if (r < B)
+            for (int k = k0; k < k1; ++k)
+              p.traj[((int64_t)k * B + r) * dim + e] =
+                  __fadd_rn(__fmul_rn(__ldg(p.out_a + k), y0), __fmul_rn(__ldg(p.out_b + k), y1));
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// SDE: at most this many warps per CTA.  At the 64 registers per thread of a 1024-thread launch bound the kernel spills
+// (ptxas -v: 36 / 68 bytes at w = 32 / 64), at 512 threads it does not.
+constexpr int kSdeMaxWarps = 16;
+
+template <int U>
+int plan_sde(int64_t B, int dim, Launch* out) {
+  const int sms = sm_count();
+  const int64_t groups = (B + RB - 1) / RB;
+  int64_t grid = 0, gpw = 0;
+  int nwarps = 4;
+  for (;; nwarps *= 2) {  // prefer more warps per CTA over several groups per warp, as plan_launch does
+    grid = (groups + nwarps - 1) / nwarps;
+    if (grid > sms) grid = sms;
+    gpw = (groups + grid * nwarps - 1) / (grid * nwarps);
+    if (gpw == 1 || nwarps == kSdeMaxWarps) break;
+  }
+  if (gpw > (1 << 19)) return 0;
+  const SdePlan pl = sde_small_plan(dim, 32 * U, nwarps, (int)gpw * RB);
+  if (pl.total > 200 * 1024) return 0;
+  out->grid = (int)grid; out->nwarps = nwarps; out->rpw = (int)gpw * RB; out->smem = pl.total;
+  return 1;
+}
+
+int plan_sde_any(int64_t B, int dim, int w, Launch* out) {
+  if (B <= 0 || dim <= 0 || dim > 1024) return 0;
+  if (w == 32) return plan_sde<1>(B, dim, out);
+  if (w == 64) return plan_sde<2>(B, dim, out);
+  return 0;  // w = 128: the two W1/W2 pairs alone take 256 KB
+}
+
+template <int U, int MAXT>
+int launch_sde_t(const SdeSmallParams& p, const Launch& L, cudaStream_t s) {
+  const void* kern = (const void*)sde_small_kernel<U, MAXT>;
+  CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+  sde_small_kernel<U, MAXT><<<L.grid, L.nwarps * 32, L.smem, s>>>(p);
+  CFM_CUDA_OK(cudaGetLastError());
+  note_launches(1);
+  return CFM_OK;
+}
+template <int U>
+int launch_sde(const SdeSmallParams& p, const Launch& L, cudaStream_t s) {
+  static_assert(kSdeMaxWarps <= 16, "the SDE kernel is instantiated for 256- and 512-thread CTAs only");
+  if (L.nwarps <= 8) return launch_sde_t<U, 256>(p, L, s);
+  return launch_sde_t<U, 512>(p, L, s);
+}
+
 }  // namespace
 
 }  // namespace cfm
@@ -711,4 +911,34 @@ extern "C" int cfm_ode_small_cnf_trajectory_f32(const float* W0, const float* b0
   return trajectory(true, "cfm_ode_small_cnf_trajectory_f32", W0, b0, W1, b1, W2, b2, W3, b3, dim, w,
                     time_varying, act, x0, batch, t_span, n_span, atol, rtol, solver, traj, state_out, workspace,
                     workspace_bytes, stream);
+}
+
+extern "C" int cfm_sde_small_supported(int64_t batch, int dim, int w) {
+  Launch L;
+  return plan_sde_any(batch, dim, w, &L);
+}
+
+extern "C" int cfm_sde_small_euler_f32(const float* const* drift_host, const float* const* score_host, int dim,
+                                       int w, int act, float sigma, const float* x0, int64_t batch, const float* grid,
+                                       int n_steps, const int* out_begin, const float* out_a, const float* out_b, int n_out,
+                                       uint64_t seed, const float* increments, float* traj, void* stream) {
+  const char* what = "cfm_sde_small_euler_f32";
+  CFM_REQUIRE(drift_host && score_host && x0 && grid && out_begin && out_a && out_b && traj, "%s: null pointer", what);
+  for (int i = 0; i < 8; ++i) CFM_REQUIRE(drift_host[i] && score_host[i], "%s: null weight pointer", what);
+  CFM_REQUIRE(n_steps >= 1 && n_out >= 2 && (act == CFM_ACT_SELU || act == CFM_ACT_SILU), "%s: bad argument", what);
+  Launch L;
+  CFM_REQUIRE(plan_sde_any(batch, dim, w, &L), "%s: unsupported shape B=%lld dim=%d w=%d", what, (long long)batch,
+              dim, w);
+  SdeSmallParams p;
+  for (int q = 0; q < 2; ++q) {
+    const float* const* n = q == 0 ? drift_host : score_host;
+    p.W0[q] = n[0]; p.b0[q] = n[1]; p.W1[q] = n[2]; p.b1[q] = n[3];
+    p.W2[q] = n[4]; p.b2[q] = n[5]; p.W3[q] = n[6]; p.b3[q] = n[7];
+  }
+  p.dim = dim; p.act = act; p.sigma = sigma; p.x0 = x0; p.B = batch;
+  p.grid = grid; p.n_steps = n_steps; p.out_begin = out_begin; p.out_a = out_a; p.out_b = out_b;
+  p.seed = seed; p.dw = increments; p.traj = traj; p.rows_per_warp = L.rpw;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (w == 32) return launch_sde<1>(p, L, s);
+  return launch_sde<2>(p, L, s);
 }

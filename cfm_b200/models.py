@@ -206,6 +206,38 @@ def _rademacher_like(x):
     return torch.randint_like(x, low=0, high=2).float() * 2 - 1.0
 
 
+class SDE(torch.nn.Module):
+    """Schrodinger-bridge SDE of the SF2M examples (examples/2D_tutorials/SF2M_tutorial.ipynb cell 5,
+    examples/single_cell/single-cell_example.ipynb cell 16): dy = [drift(t, y) + score(t, y)] dt + sigma dW, Ito, with
+    diagonal noise of constant scale sigma.
+
+    ``f`` and ``g`` are the notebooks' plain-PyTorch bodies, so they run on any device and under autograd.  Under
+    ``torch.no_grad()`` on CUDA, ``cfm_b200.sdeint`` integrates an SDE whose two nets are ``MLP(time_varying=True)``
+    of one shape in a single kernel instead (cfm_b200/sde.py)."""
+    noise_type = "diagonal"
+    sde_type = "ito"
+
+    def __init__(self, ode_drift, score, input_size=(3, 32, 32), sigma=1.0):
+        super().__init__()
+        self.drift = ode_drift
+        self.score = score
+        self.input_size = input_size
+        self.sigma = sigma
+
+    def f(self, t, y):
+        """Drift: drift(t, y) + score(t, y), with t appended as the last input column."""
+        y = y.view(-1, *self.input_size)
+        if len(t.shape) == len(y.shape):
+            x = torch.cat([y, t], 1)
+        else:
+            x = torch.cat([y, t.repeat(y.shape[0])[:, None]], 1)
+        return self.drift(x).flatten(start_dim=1) + self.score(x).flatten(start_dim=1)
+
+    def g(self, t, y):
+        """Diffusion: sigma in every component."""
+        return torch.ones_like(y) * self.sigma
+
+
 class cnf_wrapper(torch.nn.Module):
     """Continuous-normalising-flow field of the maximum-likelihood tutorial
     (examples/2D_tutorials/Maximum_likelihood_CNF_tutorial.ipynb): the state is [x, ll] with the log-density change

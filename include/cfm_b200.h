@@ -314,6 +314,25 @@ int cfm_ode_small_cnf_trajectory_f32(const float* W0, const float* b0, const flo
                                      float rtol, int solver, float* traj, cfm_rk_state* state_out,
                                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Schrodinger-bridge SDE sampling for small MLPs, ONE launch -----------------------------------------------
+ * replaces torchsde.sdeint(sde, y0, ts, method="euler") for the SDE class of the SF2M examples
+ * (examples/2D_tutorials/SF2M_tutorial.ipynb cell 5, examples/single_cell/single-cell_example.ipynb cell 16):
+ * dy = [drift(t, y) + score(t, y)] dt + sigma dW, Ito, diagonal noise, fixed-step Euler-Maruyama.
+ * drift_host, score_host: HOST arrays of 8 device pointers {W0, b0, W1, b1, W2, b2, W3, b3} each, torch.nn.Linear
+ * layout, both MLP(dim, w, time_varying=True) with out_dim == dim (time is the last input column).
+ * grid: [n_steps + 1] step times; step n is y += h f(t_n, y) + sigma dW with h = grid[n + 1] - grid[n], evaluated
+ * as fmaf(h, drift + score, y) + sigma * dW.  traj: [n_out][batch][dim]; traj[0] = x0, and output k >= 1 is
+ * out_a[k] * y_before + out_b[k] * y_after of the step n with out_begin[n] <= k < out_begin[n + 1]
+ * (out_begin: [n_steps + 1] ints).  increments (nullable): [n_steps][batch][dim] Brownian increments; when null
+ * the kernel draws dW = sqrt(h) z with z from Philox4x32-10 (counter (c / 4, row lo, row hi, n), key (seed lo,
+ * seed hi)) and Box-Muller, a function of (seed, n, row, column) only.  supported(): w in {32, 64} and the two
+ * weight sets plus the per-row state fit in shared memory. */
+int cfm_sde_small_supported(int64_t batch, int dim, int w);
+int cfm_sde_small_euler_f32(const float* const* drift_host, const float* const* score_host, int dim, int w, int act,
+                            float sigma, const float* x0, int64_t batch, const float* grid, int n_steps,
+                            const int* out_begin, const float* out_a, const float* out_b, int n_out, uint64_t seed,
+                            const float* increments, float* traj, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
