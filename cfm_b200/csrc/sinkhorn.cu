@@ -1086,6 +1086,10 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
     p.part_m = w + L.pm; p.part_s = w + L.ps; p.err_ring = reinterpret_cast<double*>(w + L.ring);
     p.mq = L.mq_bytes ? reinterpret_cast<unsigned char*>(w + L.mq) : nullptr;
   }
+  // CFM_SK_TL: timeline marks, read by both kernels (so set before the smem-staged launch)
+  static int tl = -1;
+  if (tl < 0) { const char* e = getenv("CFM_SK_TL"); tl = e ? atoi(e) : 0; }
+  p.timeline = tl;
   // precise: -1 auto, 0 fp32, 1 float64, 2 fp32 on the generic kernel, 3 float64 with fp32 exponentials ("mixed"),
   // 4 = 3 without the screening of negligible terms
   p.screen = 1;
@@ -1108,9 +1112,6 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
   const size_t vbytes = (size_t)p.n1p * 12;  // float64 stage + its fp32 copy (screened mixed mode)
   p.v_in_smem = vbytes <= 160 * 1024;
   const size_t smem = p.v_in_smem ? vbytes : 0;
-  static int tl = -1;
-  if (tl < 0) { const char* e = getenv("CFM_SK_TL"); tl = e ? atoi(e) : 0; }
-  p.timeline = tl;
   const int ng = p.n1p / 4;
   const int kg_need = (ng + kSkThreads - 1) / kSkThreads;
   if (p.vec) {

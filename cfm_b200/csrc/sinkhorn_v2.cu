@@ -82,6 +82,11 @@ __device__ __forceinline__ uint64_t v2_policy_evict_first() {
 }
 template <int NT>
 __device__ __forceinline__ void v2_consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
+__device__ __forceinline__ unsigned long long v2_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 
 // 3-byte stream: e = m*c2 - kappa in float64 (exact: a 24 x 24-bit product), quantised with one rounding and
 // clamped to [0, 2^23 - 1] (at m = cost_max the fp32 kappa may put e a rounding below 0; NaN -> 0, but a NaN cost
@@ -228,6 +233,19 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   auto may_issue = [&]() { return issued < nchunks || consumed_total != 0 || !compact; };
   if (tid == 0)
     for (int q = 0; q < S && may_issue(); ++q) issue_next();  // initial fill (wraps into the next sweep if S > nchunks)
+
+  // CFM_SK_TL (debug aid, scripts/sk_v2_timeline.py): %globaltimer marks of iteration 50 by thread 0, in the err
+  // ring region's spare tail from byte 4608 on (where sinkhorn.cu's kernel keeps its marks): [0, 6) CTA 0 and
+  // [8, 14) the last CTA (sweep start, last chunk consumed, partials stored, barrier-1 exit, combine done, barrier-2
+  // exit), [16] / [17] the earliest / latest last-chunk mark of all CTAs (factored sweep only)
+  unsigned long long* tl = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(p.err_ring) + 4608);
+  bool tl_now = false;
+  auto tl_mark = [&](int slot) {
+    if (!tl_now) return;
+    const unsigned long long t = v2_globaltimer();
+    if (slot == 1) { atomicMin(tl + 16, t); atomicMax(tl + 17, t); }
+    if (b == 0 || b == nblk - 1) tl[(b == 0 ? 0 : 8) + slot] = t;
+  };
 
   // ---- one fused sweep ----
   auto sweep = [&](bool do_row, bool do_col, const float* v_cur) {
@@ -377,6 +395,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
             }
         }
       }
+      tl_mark(1);
       consumed_total += nchunks;
       ++sweep_no;
       if (do_col) {
@@ -391,6 +410,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
                 make_float4(cs[k][0], cs[k][1], cs[k][2], cs[k][3]);
           }
       }
+      tl_mark(2);
       return;
     }
     // ---------------- log-domain sweep (span > 40): two smem reads per element ----------------
@@ -496,12 +516,18 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   };
 
   // ---- combine a slice of columns over all CTAs' partials ----
+  // 64 columns per pass.  Thread t reduces column t % 64 over the CTAs c = t / 64 (mod 8), so each load of a warp is
+  // 32 consecutive floats of one CTA's partial row (four full sectors; with 8 CTAs per warp load it was 8 sectors of
+  // 16 useful bytes each).  The 8 (max, sum) pairs of a column then meet in smem, and thread 8k folds those of column
+  // k in the order of a shuffle butterfly over 8 lanes, the order used when 8 lanes of a warp shared a column.
+  static_assert(NT == 512, "the combine maps 512 threads onto 64 columns x 8 CTA residues");
+  __shared__ float2 cpart[8][64];
   auto combine = [&](const float* v_cur, float* v_new, bool have_cur, double* err_slot) {
     double err_local = 0.0;
     const int c_begin = cslice[0], c_end = cslice[1];
-    const int sub = tid & 7;
-    for (int j0 = c_begin; j0 < c_end; j0 += (kV2Consumers >> 3)) {  // NT/8 columns per pass
-      const int j = j0 + (tid >> 3);
+    const int sub = tid >> 6;
+    for (int j0 = c_begin; j0 < c_end; j0 += 64) {
+      const int j = j0 + (tid & 63);
       const bool act = j < c_end;
       float m = -1.0e30f, s = 0.f;
       if (act) {
@@ -544,21 +570,30 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
           s = acc; m = bm;
         }
       }
-      float gm = m;
+      cpart[sub][tid & 63] = make_float2(m, s);
+      const int jf = j0 + (tid >> 3);  // the column this thread folds when tid % 8 == 0
+      const bool fold = (tid & 7) == 0 && jf < c_end;
+      const float vc = fold && have_cur ? __ldcg(v_cur + jf) : 0.f;
+      __syncthreads();
+      if (fold) {
+        float mv[8], a[8];
 #pragma unroll
-      for (int o = 4; o > 0; o >>= 1) gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, o));
-      float gs = s * ex2f(m - gm);
+        for (int l = 0; l < 8; ++l) mv[l] = cpart[l][tid >> 3].x;
+        float gm = mv[0];
 #pragma unroll
-      for (int o = 4; o > 0; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);
-      if (act && sub == 0) {
+        for (int l = 1; l < 8; ++l) gm = fmaxf(gm, mv[l]);
+#pragma unroll
+        for (int l = 0; l < 8; ++l) a[l] = __fmul_rn(cpart[l][tid >> 3].y, ex2f(mv[l] - gm));  // no FMA into the sums
+        const float gs = ((a[0] + a[4]) + (a[2] + a[6])) + ((a[1] + a[5]) + (a[3] + a[7]));
         const float vn = logb - (gm + log2f(gs));
-        v_new[j] = vn;
+        v_new[jf] = vn;
         if (have_cur) {
-          const double d = ((double)__ldcg(v_cur + j) - (double)vn) * kLn2d;
+          const double d = ((double)vc - (double)vn) * kLn2d;
           const double e = expm1(d) / (double)n1;
           err_local += e * e;
         }
       }
+      if (j0 + 64 < c_end) __syncthreads();  // cpart is rewritten by the next pass (after the last, a grid barrier follows)
     }
     if (err_slot != nullptr) {
       err_local = warp_sum(err_local);
@@ -575,6 +610,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
 
   // ---- prologue: v^0 from u = 0 ----
   if (b == 0 && tid < 4) p.err_ring[tid] = 0.0;
+  if (p.timeline && b == 0 && tid == 0) { tl[16] = ~0ull; tl[17] = 0ull; }
 
   int cur = 0, iters = 0;
   bool converged = false;
@@ -599,13 +635,18 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
     const bool last = (it == p.max_iters - 1);
     const bool check = (it % p.check_every) == 0;
     const bool do_col = !last || check;
+    tl_now = p.timeline && it == 50 && tid == 0;
+    tl_mark(0);
     sweep(true, do_col, v_work[cur]);
     iters = it + 1;
     if (!do_col) break;
     grid.sync();
+    tl_mark(3);
     if (b == 0 && tid == 0) p.err_ring[(it + 2) & 3] = 0.0;
     combine(v_work[cur], v_work[cur ^ 1], check, check ? &p.err_ring[it & 3] : nullptr);
+    tl_mark(4);
     grid.sync();
+    tl_mark(5);
     if (check) {
       err = sqrt(__ldcg(&p.err_ring[it & 3]));
       if (err < p.stop_thr) { converged = true; break; }
