@@ -28,10 +28,15 @@
 //     still reads fp32 rows and writes the copy (float64 encode, once per solve); iterations decode with no
 //     conversion instruction: the bit pattern 0x4B000000 | q is the float 2^23 + q, so e' = fmaf(F, a, -2^23 a)
 //     = fl(q*a) exactly up to the final rounding.  |e' - e| <= a/2 + ulp = span * 2^-24 + ulp; 25% fewer bytes.
+//     The 3-byte chunk (R rows of ldc bytes) is a quarter of the fp32 stage or less, so once the prologue has drained
+//     its fp32 ring the same allocation is re-carved into a kV2QStages-deep ring of 3-byte chunks and as many
+//     chunks resident for the whole solve as fit in the rest: a run of kres slab chunks in the middle of the slab,
+//     filled once, read from shared memory by every later sweep.  Only the other chunks cross the ring (and HBM).
 //   * per-CTA column partials -> [cta][n1] workspace -> grid barrier -> sliced combine -> v_new,
 //     marginal error -> grid barrier (identical to sinkhorn.cu).
 #include <stdlib.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "sinkhorn_common.cuh"
@@ -130,8 +135,19 @@ __device__ __forceinline__ int multi_row(int lane) {
   return r;
 }
 
+// Ring depth of the 3-byte stream: 2 stages leave room for 2 resident chunks at full width.  3 stages with 1 resident
+// chunk gave a slower C2 step and 4096^2 shard (DESIGN.md §3.2).
+constexpr int kV2QStages = 2;
+// Head of the dynamic shared memory, the same in every layout: the row partials [2][R][16] and the mbarriers (8 for
+// the fp32 ring, kV2QStages for the 3-byte ring, 1 for the resident chunks).  The stages follow it.
+template <int NT, int R>
+constexpr uint32_t v2_head_bytes() {
+  return (2 * R * (NT / 32) * sizeof(float2) + (8 + kV2QStages + 1) * sizeof(uint64_t) + 127) / 128 * 128;
+}
+
+// S: depth of the fp32 ring.  kres_max: 3-byte chunks that fit beside the 3-byte ring (resident chunks).
 template <int NT, int KG, int R>
-__global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, const int S) {
+__global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, int S, const int kres_max) {
   constexpr int kV2Consumers = NT, kV2Threads = NT, kV2Warps = NT / 32;
   extern __shared__ __align__(128) unsigned char v2_smem[];
   cg::grid_group grid = cg::this_grid();
@@ -147,9 +163,11 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   }
 
   const uint32_t stage_floats = (uint32_t)R * (uint32_t)n1p;
-  float* stages = reinterpret_cast<float*>(v2_smem);
-  float2* rowpart = reinterpret_cast<float2*>(stages + (size_t)S * stage_floats);  // [2][R][16]
-  uint64_t* full = reinterpret_cast<uint64_t*>(rowpart + 2 * R * kV2Warps);
+  float2* rowpart = reinterpret_cast<float2*>(v2_smem);  // [2][R][16]
+  uint64_t* const bars = reinterpret_cast<uint64_t*>(rowpart + 2 * R * kV2Warps);
+  uint64_t* full = bars;  // the ring's mbarriers: bars[0, 8) for the fp32 ring, bars[8, 8 + kV2QStages) for the 3-byte one
+  uint64_t* const res_full = bars + 8 + kV2QStages;  // the resident chunks' fill
+  float* stages = reinterpret_cast<float*>(v2_smem + v2_head_bytes<NT, R>());
   __shared__ double red[kV2Warps];
   __shared__ int cslice[2];  // this CTA's columns in the combine step (in smem: a register there would spill)
 
@@ -157,7 +175,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
     const int cpc = (n1 + nblk - 1) / nblk;
     cslice[0] = b * cpc;
     cslice[1] = min(n1, b * cpc + cpc);
-    for (int s = 0; s < S; ++s) v2_mbar_init(&full[s], 1);
+    for (int s = 0; s < 8 + kV2QStages + 1; ++s) v2_mbar_init(&bars[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -182,7 +200,9 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   const int nchunks = (nrows + R - 1) / R;
 
   // ---- ring bookkeeping (incremental: no 64-bit div/mod in the hot loop) ----
-  // chunk sequence q = 0,1,2,... over ALL sweeps; chunk q sits in stage q % S, slab chunk q % nchunks
+  // chunk sequence q = 0,1,2,... over ALL sweeps; chunk q sits in stage q % S.  Slab chunks rlo .. rlo+kres-1 are
+  // resident in smem (3-byte stream only, kres = 0 before it) and take no part in the sequence.
+  int kres = 0, rlo = 0;
   int c_st = 0;             // consumers: stage of the next chunk to consume
   uint32_t c_par = 0;       //            parity to wait for on full[c_st]
   int p_st = 0, p_chunk = 0;  // producer (thread 0): stage / slab chunk of the next chunk to issue
@@ -196,13 +216,13 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
   const int tcol = tid * 4;  // first owned column; group k adds 2048*k
   const bool full_cols = ng == kV2Consumers * KG;  // every thread owns KG valid float4 groups
 
-  // L2 residency: the first `resident` chunks of every slab are loaded evict_last (they stay in the
+  // L2 residency: the streamed chunks of every slab below `l2_end` are loaded evict_last (they stay in the
   // L2 from sweep to sweep), the rest evict_first (pure streaming): only the streaming part
   // crosses HBM every iteration.  p.l2_resident_frac <= 0 leaves the default policy.
-  // The 3-byte stream keeps the same resident BYTES (more chunks of the smaller rows); its fp32 prologue is read
-  // once and streams entirely.
-  // (`resident` switches to the 3-byte stream's value when the producer switches format, see below)
-  int resident = p.l2_resident_frac <= 0.f ? -1 : compact ? 0 : (int)(p.l2_resident_frac * (float)nchunks);
+  // The 3-byte stream keeps the same L2-resident BYTES (more chunks of the smaller rows) in the chunks that follow
+  // the smem-resident ones; its fp32 prologue is read once and streams entirely.
+  // (`l2_end` switches to the 3-byte stream's value when the producer switches format, see below)
+  int l2_end = p.l2_resident_frac <= 0.f ? -1 : compact ? 0 : (int)(p.l2_resident_frac * (float)nchunks);
   // thread 0: issue the bulk copies of the next chunk into its (free) stage
   auto issue_next = [&]() {
     const int r0 = r_begin + p_chunk * R;
@@ -210,20 +230,22 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
     const bool q = compact && issued >= nchunks;  // the first nchunks chunks are the prologue's
     const uint32_t ldc = (uint32_t)p.ldc;
     const uint32_t row_bytes = q ? ldc : (uint32_t)n1 * 4u;
-    const uint64_t pol = p_chunk < resident ? v2_policy_evict_last() : v2_policy_evict_first();
+    const uint32_t pitch = q ? ldc : (uint32_t)n1p * 4u;  // a stage is R rows at this pitch
+    const uint64_t pol = p_chunk < l2_end ? v2_policy_evict_last() : v2_policy_evict_first();
     v2_mbar_expect_tx(&full[p_st], (uint32_t)rv * row_bytes);
     for (int r = 0; r < rv; ++r) {
-      unsigned char* dst = reinterpret_cast<unsigned char*>(stages + (size_t)p_st * stage_floats) +
-                           (size_t)r * (q ? ldc : (uint32_t)n1p * 4u);
+      unsigned char* dst = reinterpret_cast<unsigned char*>(stages) + ((size_t)p_st * R + r) * pitch;
       const void* src = q ? static_cast<const void*>(p.mq + (int64_t)(r0 + r) * ldc)
                           : static_cast<const void*>(p.M + (int64_t)(r0 + r) * p.ldm);
-      if (resident < 0) v2_bulk_load(dst, src, row_bytes, &full[p_st]);
+      if (l2_end < 0) v2_bulk_load(dst, src, row_bytes, &full[p_st]);
       else v2_bulk_load_hint(dst, src, row_bytes, &full[p_st], pol);
     }
     ++issued;
     p_chunk += p_dir;
-    if (p_chunk == nchunks) { p_chunk = nchunks - 1; p_dir = -1; }   // next sweep runs backwards
-    else if (p_chunk < 0) { p_chunk = 0; p_dir = 1; }
+    if (p_chunk >= rlo && p_chunk < rlo + kres) p_chunk = p_dir > 0 ? rlo + kres : rlo - 1;  // skip the resident run
+    // at either end of the slab the next sweep runs the other way and starts with the chunk this one ended on
+    if (p_chunk >= nchunks) { p_chunk = rlo + kres < nchunks ? nchunks - 1 : rlo - 1; p_dir = -1; }
+    else if (p_chunk < 0) { p_chunk = rlo > 0 ? 0 : rlo + kres; p_dir = 1; }
     if (++p_st == S) p_st = 0;
   };
   // The ring runs S chunks ahead across sweeps, and the prologue's last S chunks are iteration 0's first: their
@@ -282,10 +304,13 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
         const int chunk = (sweep_no & 1) ? nchunks - 1 - cc : cc;
         const int r0 = r_begin + chunk * R;
         const int rv = min(R, r_begin + nrows - r0);
+        const bool res = (unsigned)(chunk - rlo) < (unsigned)kres;  // resident: slot S + chunk - rlo, past the ring
         const float* sbase = stages + (uint32_t)c_st * stage_floats + tcol;
-        const unsigned char* qbase = reinterpret_cast<const unsigned char*>(stages + (uint32_t)c_st * stage_floats) + 12 * tid;
+        const unsigned char* qbase =
+            reinterpret_cast<const unsigned char*>(stages) + (uint32_t)(res ? S + chunk - rlo : c_st) * R * ldc + 12 * tid;
         float2* rp = rowpart + (cc & 1) * R * kV2Warps;
-        v2_mbar_wait(&full[c_st], c_par);
+        if (res) v2_mbar_wait(res_full, 0);
+        else v2_mbar_wait(&full[c_st], c_par);
         float4 E[R][KG];
         // E of every owned group of the stage; ALL: every thread owns KG valid groups of R rows (no predicates)
         auto form_E = [&](auto FMT, auto ALL) {
@@ -334,7 +359,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
         const bool all = full_cols && rv == R;  // common case: no predicates in the hot loop
         if (fmt == 2) { if (all) form_E(std::integral_constant<int, 2>{}, kT{}); else form_E(std::integral_constant<int, 2>{}, kF{}); }
         else { if (all) form_E(std::integral_constant<int, 0>{}, kT{}); else form_E(std::integral_constant<int, 0>{}, kF{}); }
-        if (++c_st == S) { c_st = 0; c_par ^= 1u; }
+        if (!res && ++c_st == S) { c_st = 0; c_par ^= 1u; }
         if (do_row) {
           float sr[R];
 #pragma unroll
@@ -353,7 +378,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
         // every warp has now copied its part of the stage into registers: after this barrier the
         // stage is free, so thread 0 refills it with the chunk S positions ahead
         v2_consumer_barrier<NT>();
-        if (tid == 0 && may_issue()) issue_next();
+        if (tid == 0 && !res && may_issue()) issue_next();
         float U[R];
         if (do_row) {
           // fold the 16 per-warp partials: lanes 0-15 take row r, lanes 16-31 row r+1 (one tree for two rows)
@@ -396,7 +421,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
         }
       }
       tl_mark(1);
-      consumed_total += nchunks;
+      consumed_total += nchunks - kres;
       ++sweep_no;
       if (do_col) {
         // sum_i ex2(M c2 + u_i) over this slab = cs * 2^(kappa + uref): partial (max, sum) form
@@ -621,10 +646,31 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
     // proxy.  Each slab is written and read by its own CTA only, so a CTA barrier suffices.
     asm volatile("fence.proxy.async.global;" ::: "memory");
     __syncthreads();
+    // The fp32 ring is drained (no 3-byte chunk is issued before this point): re-carve its memory into the 3-byte
+    // ring and the resident chunks behind it, each stage and chunk R rows of ldc bytes.  The resident run sits in
+    // the middle of the slab: there the ring's copies are in flight while the consumers read it, so HBM stays busy.
+    // (At either end of a sweep the ring is already full, and every CTA would read its resident chunks at the same
+    // time while HBM idles.)
+    S = kV2QStages;
+    full = bars + 8;
+    c_st = 0; c_par = 0; p_st = 0;
+    kres = min(kres_max, nchunks);
+    rlo = (nchunks - kres) / 2;
     if (tid == 0) {
-      if (resident >= 0)
-        resident = min(nchunks, (int)(p.l2_resident_frac * (float)nchunks * (4.f * (float)n1) / (float)p.ldc));
-      while (issued < consumed_total + S) issue_next();
+      const uint32_t ldc = (uint32_t)p.ldc;
+      if (kres > 0) {
+        const int rows = min(nrows - rlo * R, kres * R);
+        v2_mbar_expect_tx(res_full, (uint32_t)rows * ldc);
+        for (int r = 0; r < rows; ++r)
+          v2_bulk_load(reinterpret_cast<unsigned char*>(stages) + ((size_t)S * R + r) * ldc,
+                       p.mq + (int64_t)(r_begin + rlo * R + r) * ldc, ldc, res_full);
+      }
+      if (l2_end >= 0) {  // the first streamed chunks of the slab, as many as the fp32 share's bytes
+        const int l2c = (int)(p.l2_resident_frac * (float)nchunks * (4.f * (float)n1) / (float)ldc);
+        l2_end = min(nchunks, l2c <= rlo ? l2c : l2c + kres);
+      }
+      if (kres < nchunks)
+        while (issued < consumed_total + S) issue_next();
     }
   }
   grid.sync();
@@ -664,6 +710,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
       v2_mbar_wait(&full[c_st], c_par);
       if (++c_st == S) { c_st = 0; c_par ^= 1u; }
     }
+    if (kres > 0) v2_mbar_wait(res_full, 0);
   }
 
   for (int j = b * kV2Threads + tid; j < n1; j += nblk * kV2Threads)
@@ -684,20 +731,41 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, co
 template <int NT, int KG, int R>
 static int v2_launch_t(SkParams& p, cudaStream_t s) {
   auto kern = sinkhorn_v2_kernel<NT, KG, R>;
+  // dynamic shared memory: what a block may opt in to, less the kernel's static shared memory
+  // (the static size is a property of the compiled kernel: queried once, it costs the small solves host time)
+  static size_t static_smem = 0;
+  if (static_smem == 0) {
+    cudaFuncAttributes fa;
+    CFM_CUDA_OK(cudaFuncGetAttributes(&fa, kern));
+    static_smem = fa.sharedSizeBytes;
+  }
+  int dev = 0, optin = 0;
+  CFM_CUDA_OK(cudaGetDevice(&dev));
+  CFM_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const size_t head = v2_head_bytes<NT, R>();
+  const size_t budget = (size_t)optin - static_smem;
   const size_t stage_bytes = (size_t)R * p.n1p * 4;
-  const size_t fixed = (size_t)2 * R * (NT / 32) * sizeof(float2) + 8 * sizeof(uint64_t) + 128;
-  const size_t budget = 220 * 1024;
-  if (budget < fixed + 2 * stage_bytes) return 1;
-  int S = (int)((budget - fixed) / stage_bytes);
+  if (budget < head + 2 * stage_bytes) return 1;
+  int S = (int)((budget - head) / stage_bytes);
   if (S > 8) S = 8;
-  const size_t smem = (size_t)S * stage_bytes + fixed;
+  int grid = sm_count();
+  if (grid > p.n0) grid = p.n0;
+  // the 3-byte stream re-carves the prologue's ring: kV2QStages stages, then as many resident chunks as fit (no
+  // more than the longest slab has)
+  size_t ring = (size_t)S * stage_bytes;
+  int kres_max = 0;
+  if (p.mq != nullptr) {
+    const size_t qchunk = (size_t)R * p.ldc;
+    const int slab_chunks = ((p.n0 + grid - 1) / grid + R - 1) / R;
+    kres_max = std::max(0, std::min(slab_chunks, (int)((budget - head) / qchunk) - kV2QStages));
+    ring = std::max(ring, (size_t)(kV2QStages + kres_max) * qchunk);
+  }
+  const size_t smem = ring + head;
   CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 0;
   CFM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, NT, smem));
   if (per_sm < 1) return 1;
-  int grid = sm_count();
-  if (grid > p.n0) grid = p.n0;
-  void* args[] = {(void*)&p, (void*)&S};
+  void* args[] = {(void*)&p, (void*)&S, (void*)&kres_max};
   CFM_CUDA_OK(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(NT), args, smem, s));
   note_launches(1);
   return CFM_OK;
