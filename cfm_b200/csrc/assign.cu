@@ -6,18 +6,25 @@
 // (POT casts M to float64); so does this kernel.
 //
 // Algorithm: shortest augmenting paths with dual variables (Jonker-Volgenant / Crouse form).
-//   init   u_i = min_j c_ij, greedy matching on the argmin columns (keeps complementary slackness)
+//   init   u_i = min_j c_ij, greedy matching on the argmin columns (keeps complementary slackness;
+//          assign_fast_kernel adds a column reduction and a second claim, see there)
 //   then for every still-free row: Dijkstra over columns on reduced costs c_ij - u_i - v_j,
 //   dual update, augmentation.  The optimum is unique almost surely for continuous data, so the
 //   result equals the reference's sigma bit for bit; ties are broken deterministically
 //   (free column first, then lowest index).
 //
 // GPU mapping: the problem at the reference's sizes (n = 128..256, BASELINE config 1) is a
-// 256 KB latency-bound graph search, not a bandwidth problem.  One CTA runs the whole solve with
-// every per-column array (v, shortest, path, row4col, scanned flags) resident in shared memory;
-// each Dijkstra step is one coalesced row read of M (L2 resident) + one block-wide argmin
-// (warp shuffles + one smem hop).  No host round trips: sigma stays on the device for the
-// sampling kernel.
+// 256 KB latency-bound graph search, not a bandwidth problem.  One CTA runs the whole solve; each
+// Dijkstra step is one coalesced row read of M + one block-wide argmin (warp shuffles + one smem
+// hop).  No host round trips: sigma stays on the device for the sampling kernel.
+// cfm_assign_exact_f32 picks the code path from n alone:
+//   n <= 4096          assign_fast_kernel<KCB>, nt = max(64, round32(n)) <= 1024 threads, KCB = 1, 2 or 4
+//                      columns per thread (n = 2049..3072: column slot 3 is padding on every thread),
+//                      per-column state in registers, and the first cache_rows rows of M staged in shared
+//                      memory (every row up to n = 222, 4 rows at n = 4096)
+//   4097 <= n <= 5534  assign_kernel with u and every per-column array (v, shortest, path, row4col, srlist,
+//                      scanned flags) in shared memory: 37 n + 16 bytes <= 200 KB
+//   n >= 5535          assign_kernel with all of them in the global workspace
 #include <float.h>
 
 #include "common.cuh"
@@ -242,8 +249,11 @@ __device__ __forceinline__ IKey ikey_min(const IKey& a, const IKey& b) {
 }
 
 // ---- the general fast path (n <= 4096): whole CTA, thread t owns columns t, t + nt, ... (KCB of them) ------
-// Same algorithm, initialisation and tie-breaking as assign_kernel (hence the same sigma), reformulated so that
-// every warp executes as few instructions per Dijkstra step as possible -- a lone warp retires one dependent
+// The same shortest augmenting paths and Dijkstra tie-breaking as assign_kernel, with a stronger greedy start (the
+// row reduction, then a column reduction and a second claim per free column) and reduced costs evaluated as
+// (minval - u_i) + (c_ij - v_j).  So the two kernels return the same sigma only where the optimum is unique (almost
+// surely for continuous costs).  Reformulated so that every warp executes as few instructions per Dijkstra step as
+// possible -- a lone warp retires one dependent
 // instruction every few cycles, so the step time IS the per-warp instruction count.  Per-column state (dual v, shortest label, predecessor, scanned / free bits)
 // lives in registers; labels are kept as integer-orderable images of the float64 values (dkey) so that the hot
 // loop is branch-free integer selects -- lanes disagree on every predicate, and divergent float64 compares were

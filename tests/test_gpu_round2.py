@@ -162,9 +162,14 @@ def test_status_is_evaluated_with_warn_false(capsys):
 def test_exact_ot_unequal_batch_sizes_vs_lp_oracle(n0, n1, d):
     """pot.emd takes marginals of any two sizes (reference :79,87).  The device solves the lcm(n0, n1)-replicated
     assignment problem; the oracle solves the transport LP itself (SciPy HiGHS): same plan, same cost."""
+    _unequal_batch_sizes_vs_lp(OTPlanSampler("exact"), n0, n1, d)
+
+
+def _unequal_batch_sizes_vs_lp(s, n0, n1, d):
+    """get_map, wasserstein and sample_plan of the exact sampler ``s`` between seeded batches of n0 and n1 points
+    against the transport LP."""
     g = torch.Generator().manual_seed(n0 * 1000 + n1)
     x0, x1 = torch.randn(n0, d, generator=g), torch.randn(n1, d, generator=g)
-    s = OTPlanSampler("exact")
     P = s.get_map(x0.to(DEV), x1.to(DEV))
     M = oc.cost_matrix(x0, x1).numpy()
     G = oot.emd(oot.unif(n0), oot.unif(n1), M)
