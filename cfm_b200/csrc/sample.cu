@@ -197,8 +197,88 @@ struct RowWeight {
   }
 };
 
+// Last column of [b0, bend) whose weight is positive, or -1.  Only the rare walks that reach the end of a block or of
+// the row without crossing their target call it.
+template <bool F64>
+__device__ __forceinline__ int last_positive(const RowWeight<F64>& W, int b0, int bend, bool vec, int lane) {
+  int jl = -1;
+  if (vec) {
+    for (int j = b0 + lane * 4; j < bend; j += 128) {
+      const float4 w = W.four(j);
+      jl = w.w > 0.f ? j + 3 : w.z > 0.f ? j + 2 : w.y > 0.f ? j + 1 : w.x > 0.f ? j : jl;
+    }
+  } else {
+    for (int j = b0 + lane; j < bend; j += 32) if (W.one(j) > 0.f) jl = j;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) jl = max(jl, __shfl_xor_sync(0xffffffffu, jl, o));
+  return jl;
+}
+
+// pass B: coarse blocks of 1024 columns, then a fine scan inside the block whose sum crosses `target`.  Returns the
+// column, or -1 when the row ends without crossing; `run` is then the sum of all the row's weights.
+template <bool F64>
+__device__ __forceinline__ int walk_row(const RowWeight<F64>& W, int n1, bool vec, double target, int lane,
+                                        double& run) {
+  run = 0.0;
+  for (int b0 = 0; b0 < n1; b0 += 1024) {
+    const int bend = min(n1, b0 + 1024);
+    double bp = 0.0;
+    if (vec) {
+      for (int j = b0 + lane * 4; j < bend; j += 128) { const float4 w = W.four(j); bp += (double)((w.x + w.y) + (w.z + w.w)); }
+    } else {
+      for (int j = b0 + lane; j < bend; j += 32) bp += (double)W.one(j);
+    }
+    const double bsum = warp_sum(bp);
+    if (!(run + bsum > target)) { run += bsum; continue; }
+    // fine scan: 128 (vec) or 32 (scalar) columns per step, in natural column order
+    const int step = vec ? 128 : 32;
+    for (int j0 = b0; j0 < bend; j0 += step) {
+      float w[4] = {0.f, 0.f, 0.f, 0.f};
+      const int j = j0 + (vec ? lane * 4 : lane);
+      if (j < bend) {
+        if (vec) { const float4 q = W.four(j); w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w; }
+        else w[0] = W.one(j);
+      }
+      const double mine = (double)((w[0] + w[1]) + (w[2] + w[3]));
+      double incl = mine;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const double t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      const bool hit = (j < bend) && (run + incl > target);
+      const unsigned ballot = __ballot_sync(0xffffffffu, hit);
+      if (ballot) {
+        const int src = __ffs(ballot) - 1;
+        // the winning lane resolves the element inside its float4; if the element-wise float64 sum ends a rounding
+        // short of the fp32 group sum, the group's last element of positive weight is the draw
+        int jj = -1;
+        if (lane == src) {
+          double r2 = run + incl - mine;
+          const int cnt = vec ? 4 : 1;
+          for (int c = 0; c < cnt; ++c) {
+            if (w[c] > 0.f) jj = j + c;
+            r2 += (double)w[c];
+            if (r2 > target) { jj = j + c; break; }
+          }
+        }
+        return __shfl_sync(0xffffffffu, jj, src);
+      }
+      run += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    // the block's sum crossed the target but the in-order scan, summed in another order, ended a rounding short:
+    // the target sits at the block's end, whose last weighted column is the draw (never a column of weight 0)
+    const int jl = last_positive(W, b0, bend, vec, lane);
+    return jl >= 0 ? jl : bend - 1;
+  }
+  return -1;
+}
+
 // known_total > 0: the row's mass is known analytically (1/n0: the weights are the plan entries and the potentials'
 // last update was the row update), so the totalling pass over the row is skipped -- one pass less over 32 KB per draw.
+// The weights' own sum differs from it by their rounding (~1e-6 relative): a walk that runs off the row's end is
+// repeated against the sum it measured, so the draw never lands on a column of weight 0.
 template <bool F64>
 __device__ __forceinline__ int draw_in_row(RowWeight<F64>& W, bool have_shift, int n1, bool vec, double frac,
                                            int lane, int32_t* status, double known_total) {
@@ -221,67 +301,19 @@ __device__ __forceinline__ int draw_in_row(RowWeight<F64>& W, bool have_shift, i
     }
     total = warp_sum(part);
   }
-  int jsel = -1;
   if (!(total > 0.0) || !isfinite(total)) {
     if (lane == 0 && status) atomicOr(status, CFM_FLAG_NONFINITE);
     return min(n1 - 1, (int)(frac * (double)n1));
   }
-  const double target = frac * total;
-  double run = 0.0;
-  // pass B: coarse blocks of 1024 columns, then a fine scan inside the block that crosses
-  for (int b0 = 0; b0 < n1 && jsel < 0; b0 += 1024) {
-    const int bend = min(n1, b0 + 1024);
-    double bp = 0.0;
-    if (vec) {
-      for (int j = b0 + lane * 4; j < bend; j += 128) { const float4 w = W.four(j); bp += (double)((w.x + w.y) + (w.z + w.w)); }
-    } else {
-      for (int j = b0 + lane; j < bend; j += 32) bp += (double)W.one(j);
-    }
-    const double bsum = warp_sum(bp);
-    if (run + bsum > target || bend == n1) {
-      // fine scan: 128 (vec) or 32 (scalar) columns per step, in natural column order
-      const int step = vec ? 128 : 32;
-      for (int j0 = b0; j0 < bend && jsel < 0; j0 += step) {
-        float w[4] = {0.f, 0.f, 0.f, 0.f};
-        const int j = j0 + (vec ? lane * 4 : lane);
-        if (j < bend) {
-          if (vec) { const float4 q = W.four(j); w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w; }
-          else w[0] = W.one(j);
-        }
-        const double mine = (double)((w[0] + w[1]) + (w[2] + w[3]));
-        double incl = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const double t = __shfl_up_sync(0xffffffffu, incl, o);
-          if (lane >= o) incl += t;
-        }
-        const bool hit = (j < bend) && (run + incl > target);
-        const unsigned ballot = __ballot_sync(0xffffffffu, hit);
-        if (ballot) {
-          const int src = __ffs(ballot) - 1;
-          // the winning lane resolves the element inside its float4
-          int jj = -1;
-          if (lane == src) {
-            double r2 = run + incl - mine;
-            const int cnt = vec ? 4 : 1;
-            jj = j + cnt - 1;
-            for (int c = 0; c < cnt; ++c) { r2 += (double)w[c]; if (r2 > target) { jj = j + c; break; } }
-          }
-          jsel = __shfl_sync(0xffffffffu, jj, src);
-        }
-        run += __shfl_sync(0xffffffffu, incl, 31);
-      }
-      if (jsel < 0) {  // rounding at the very end of the row -- or NaN weights, which never cross the target
-        if (!(run == run) && lane == 0 && status) atomicOr(status, CFM_FLAG_NONFINITE);
-        jsel = bend - 1;
-      }
-    } else {
-      run += bsum;
-    }
-  }
-  if (jsel < 0) {
-    if (!(run == run) && lane == 0 && status) atomicOr(status, CFM_FLAG_NONFINITE);  // NaN weights (known-total path)
-    jsel = n1 - 1;
+  double run;
+  int jsel = walk_row(W, n1, vec, frac * total, lane, run);
+  // no crossing: the weights sum to less than the total the target was taken from.  Invert against their own sum,
+  // which the second walk adds up in the same order (it crosses unless frac rounds to 1)
+  if (jsel < 0 && run > 0.0) jsel = walk_row(W, n1, vec, frac * run, lane, run);
+  if (jsel < 0) {  // frac == 1, or NaN weights, which never cross the target
+    if (!(run == run) && lane == 0 && status) atomicOr(status, CFM_FLAG_NONFINITE);
+    jsel = last_positive(W, 0, n1, vec, lane);
+    if (jsel < 0) jsel = n1 - 1;
   }
   return jsel;
 }
@@ -317,9 +349,13 @@ __global__ void draw_uniform_rows_kernel(const float* __restrict__ M, int n0, in
   const bool precise = cost_max ? !((normalize ? 1.f : cmax) / reg <= 64.f) : true;
   int jsel;
   // with log_u the weights are pi_ij and their row sum is a_i = 1/n0 (row update last): no totalling pass.  A
-  // potential pair that is not finite (NaN costs) falls back to the measured total, which flags it.
+  // potential pair that is not finite (NaN costs) falls back to the measured total, which flags it.  So does a solve
+  // in fp32 arithmetic (status[2] == 0, precision="fp32") at |M/reg| > 64: its fp32 exponents of magnitude up to
+  // |M/reg| move the row masses of the precise weights further from 1/n0 than their own rounding does.
   const double lui = lu ? lu[i] : 0.0;
-  const double known = (lu != nullptr && lui == lui && fabs(lui) < 1.0e300) ? 1.0 / (double)n0 : -1.0;
+  const bool fp32_solve_precise_draw = precise && status != nullptr && status[2] == 0;
+  const double known = (lu != nullptr && lui == lui && fabs(lui) < 1.0e300 && !fp32_solve_precise_draw)
+                           ? 1.0 / (double)n0 : -1.0;
   if (precise) {
     RowWeight<true> W{row, lv, c2, reg, cmax, normalize, 0.f, lui};
     jsel = draw_in_row<true>(W, lu != nullptr, n1, vec, frac, lane, status, known);

@@ -117,6 +117,9 @@ int cfm_plan_dot_cost(const float* M, int n0, int n1, int64_t ldm, float reg,
  * pass is skipped and the within-row inversion weighs column j by pi_ij itself (exponent
  * -M_ij/reg + log_u_i + log_v_j <= 0: no under/overflow at any |M/reg|; formed in fp32 when
  * |M/reg| <= 64 and with float64 adds beyond, the rule cfm_sinkhorn_log_f32's auto mode uses).
+ * A walk whose target lies past the weights' own sum is repeated against that sum, and the
+ * row is totalled first when status[2] == 0 (fp32 solve) and |M/reg| > 64, so the draw is
+ * never a column of weight 0.
  */
 size_t cfm_plan_sample_workspace_bytes(int n0);
 int cfm_plan_sample(const float* M, int n0, int n1, int64_t ldm, float reg,
