@@ -82,6 +82,9 @@ SIGNATURES = {
     "cfm_sde_small_supported": (_i, [_i64, _i, _i]),
     "cfm_sde_small_euler_f32": (_i, [_p, _p, _i, _i, _i, _f, _p, _i64, _p, _i, _p, _p, _p, _i, C.c_uint64, _p, _p,
                                      _p]),
+    "cfm_mlp_small_train_supported": (_i, [_i64, _i, _i, _i]),
+    "cfm_mlp_small_train_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
+    "cfm_mlp_small_mse_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),
 }
 
 _lock = threading.Lock()

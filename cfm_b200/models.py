@@ -5,8 +5,9 @@
 checkpoints load unchanged.  Under ``torch.no_grad()`` on a CUDA device -- the regime of the ODE
 sampling loop, where torchdyn calls ``forward(t, x)`` six times per step
 (examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb:332-338) -- the forward runs
-in libcfm_b200's kernels (cfm_mlp_forward_f32).  With autograd enabled (training) the module is an
-ordinary ``torch.nn.Sequential``: the backward pass is outside the north_star hot path.
+in libcfm_b200's kernels (cfm_mlp_forward_f32).  With autograd enabled the module is an ordinary
+``torch.nn.Sequential`` on any device; the tutorials' training step (forward, regression loss and backward of a small
+``MLP(time_varying=True)``) runs in one kernel through ``cfm_b200.flow_matching_loss`` instead (cfm_b200/train.py).
 """
 import torch
 
@@ -114,8 +115,8 @@ class MLP(torch.nn.Module):
 
     def _use_kernels(self, x):
         """Sampling regime (no autograd): the kernels, or nothing -- a CPU tensor under ``torch.no_grad()`` raises
-        instead of silently running ``torch.nn.Sequential`` (north_star: no CPU fallback).  With autograd enabled
-        (training; the backward pass is outside the hot path) the module is plain PyTorch on any device."""
+        instead of silently running ``torch.nn.Sequential`` (north_star: no CPU fallback).  With autograd enabled the
+        module is plain PyTorch on any device (the device training step is ``cfm_b200.flow_matching_loss``)."""
         if torch.is_grad_enabled():
             return False
         if not x.is_cuda:

@@ -1,0 +1,121 @@
+"""The training step of the 2-D tutorials on the device: drop-in for the three lines every training cell repeats,
+
+    vt = model(torch.cat([xt, t[:, None]], dim=-1))
+    loss = torch.mean((vt - ut) ** 2)
+    loss.backward()
+
+(examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb raw lines 166-186, 310-330, 458-479, 602-623;
+Flow_matching_tutorial.ipynb and SF2M_tutorial.ipynb likewise), as
+
+    loss = cfm_b200.flow_matching_loss(model, xt, t, ut)
+    loss.backward()
+
+ONE kernel (csrc/train_small.cu) computes the loss and the gradients of all eight parameters; ``loss`` is attached to
+the autograd graph of the parameters, so ``backward()``, gradient accumulation, clipping, any ``torch.optim``
+optimizer and DDP hooks work as with the eager lines.  The SF2M score loss
+``torch.mean((lambda_t[:, None] * score_model(...) + eps) ** 2)`` is
+``flow_matching_loss(score_model, xt, t, -eps, row_scale=lambda_t)``.
+
+Only the tutorial class of model is accelerated: ``cfm_b200.MLP(time_varying=True)`` with ``w`` in {32, 64},
+``dim <= 8`` and ``out_dim <= 8``, fp32 on a CUDA device.  Anything else raises -- there is no eager fallback
+(``MLP.forward`` under autograd is still plain PyTorch for whoever wants it).  Gradients flow to the parameters only.
+"""
+import torch
+from torch.autograd.function import once_differentiable
+
+from . import _ffi
+from .models import MLP
+
+
+def _launch(model, params, xt, t, ut, row_scale, with_grad):
+    """One library call: (loss 0-d, flat gradient buffer in parameters() order or None)."""
+    L = _ffi.lib()
+    dev = xt.device
+    B = xt.shape[0]
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    grads = torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev) if with_grad else None
+    ws = _ffi.workspace(L.cfm_mlp_small_train_workspace_bytes(B, model.dim, model.w, model.out_dim), dev)
+    with torch.cuda.device(dev):  # kernels launch on the current device: make it the tensors' one
+        _ffi.check(L.cfm_mlp_small_mse_grad_f32(
+            *[_ffi.ptr(p) for p in params], model.dim, model.w, model.out_dim, model.act, _ffi.ptr(xt), _ffi.ptr(t),
+            _ffi.ptr(ut), _ffi.ptr(row_scale), B, 1 if with_grad else 0, _ffi.ptr(loss), _ffi.ptr(grads),
+            _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)), "cfm_mlp_small_mse_grad_f32")
+    return loss, grads
+
+
+class _MseGrad(torch.autograd.Function):
+    """loss(parameters): forward computes the loss and, in the same launch, its gradients for upstream gradient 1;
+    backward scales that flat buffer by ``grad_output`` and hands out views of it."""
+
+    @staticmethod
+    def forward(ctx, model, xt, t, ut, row_scale, *params):
+        loss, grads = _launch(model, [p.detach().contiguous() for p in params], xt, t, ut, row_scale, True)
+        ctx.grads = grads
+        ctx.shapes = [p.shape for p in params]
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        flat = ctx.grads * grad_output
+        out, o = [], 0
+        for shape in ctx.shapes:
+            n = shape.numel()
+            out.append(flat[o:o + n].view(shape))
+            o += n
+        return (None, None, None, None, None, *out)
+
+
+def _check_model(model):
+    if not isinstance(model, MLP):
+        raise NotImplementedError(
+            f"flow_matching_loss: no training kernel for {type(model).__name__}; it takes "
+            "cfm_b200.MLP(time_varying=True) with w in {32, 64}, dim <= 8, out_dim <= 8")
+    if not (model.time_varying and model.w in (32, 64) and 1 <= model.dim <= 8 and 1 <= model.out_dim <= 8
+            and model.act in (_ffi.ACT_SELU, _ffi.ACT_SILU)):
+        raise NotImplementedError(
+            f"flow_matching_loss: no training kernel for MLP(dim={model.dim}, out_dim={model.out_dim}, w={model.w}, "
+            f"time_varying={model.time_varying}, act={model.act}); the kernel's class is w in {{32, 64}}, dim <= 8, "
+            "out_dim <= 8, time_varying=True, SELU or SiLU")
+
+
+def flow_matching_loss(model, xt, t, ut, row_scale=None):
+    """``torch.mean((s[:, None] * model(torch.cat([xt, t[:, None]], -1)) - ut) ** 2)`` with ``s = row_scale`` (or 1),
+    as a 0-d fp32 CUDA tensor.
+
+    ``xt`` (B, dim), ``t`` (B,), ``ut`` (B, out_dim), ``row_scale`` (B,): fp32 on the parameters' CUDA device.  With
+    autograd enabled the result carries the gradients of the model's eight parameters (computed in the same launch as
+    the loss); under ``torch.no_grad()`` the kernel computes the loss only, with the same bits."""
+    _check_model(model)
+    tensors = [("xt", xt), ("t", t), ("ut", ut)] + ([("row_scale", row_scale)] if row_scale is not None else [])
+    for name, v in tensors:
+        if not torch.is_tensor(v):
+            raise ValueError(f"flow_matching_loss: {name} must be a tensor; got {type(v).__name__}")
+        if v.requires_grad:
+            raise ValueError(f"flow_matching_loss: {name} requires grad, but gradients flow to the model's parameters "
+                             "only; detach it")
+    if xt.dim() != 2 or xt.shape[1] != model.dim or xt.shape[0] < 1:
+        raise ValueError(f"flow_matching_loss: xt must be (B >= 1, {model.dim}); got {tuple(xt.shape)}")
+    B = xt.shape[0]
+    if tuple(t.shape) != (B,):
+        raise ValueError(f"flow_matching_loss: t must be ({B},), one time per row; got {tuple(t.shape)}")
+    if tuple(ut.shape) != (B, model.out_dim):
+        raise ValueError(f"flow_matching_loss: ut must be ({B}, {model.out_dim}); got {tuple(ut.shape)}")
+    if row_scale is not None and tuple(row_scale.shape) != (B,):
+        raise ValueError(f"flow_matching_loss: row_scale must be ({B},); got {tuple(row_scale.shape)}")
+    params = [p for lin in model._linears() for p in (lin.weight, lin.bias)]
+    dev = params[0].device
+    if dev.type != "cuda" or any(p.device != dev or p.dtype != torch.float32 for p in params):
+        raise _ffi.CfmLibraryError("flow_matching_loss: the MLP's parameters must be fp32 on one CUDA device (there "
+                                   "is no CPU fallback; the eager lines run anywhere)")
+    for name, v in tensors:
+        if v.device != dev or v.dtype != torch.float32:
+            raise _ffi.CfmLibraryError(f"flow_matching_loss: {name} must be fp32 on the parameters' device {dev}; got "
+                                       f"{v.dtype} on {v.device}")
+    xt, t, ut = xt.contiguous(), t.contiguous(), ut.contiguous()
+    if row_scale is not None:
+        row_scale = row_scale.contiguous()
+    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+        return _MseGrad.apply(model, xt, t, ut, row_scale, *params)
+    loss, _ = _launch(model, [p.detach().contiguous() for p in params], xt, t, ut, row_scale, False)
+    return loss

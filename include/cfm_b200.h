@@ -350,6 +350,30 @@ int cfm_sde_small_euler_f32(const float* const* drift_host, const float* const* 
                             const int* out_begin, const float* out_a, const float* out_b, int n_out, uint64_t seed,
                             const float* increments, float* traj, void* stream);
 
+/* ---- training step of small vector-field MLPs: the regression loss and all parameter gradients, ONE launch ------
+ * replaces the three lines every training cell of the 2-D tutorials repeats per step
+ * (examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb raw lines 166-186, 310-330, 458-479, 602-623;
+ * Flow_matching_tutorial.ipynb and SF2M_tutorial.ipynb likewise):
+ *     vt = model(torch.cat([xt, t[:, None]], dim=-1)); loss = torch.mean((vt - ut) ** 2); loss.backward()
+ * for model = MLP(dim, out_dim, w, time_varying=True).  Computes
+ *     *loss = mean over [batch][out_dim] of (row_scale[r] * MLP([x_r, t_r]) - target[r])^2     (row_scale null: 1)
+ * and, when with_grad != 0, d loss / d parameter into grads: W0 [w][dim + 1], b0 [w], W1 [w][w], b1, W2 [w][w], b2,
+ * W3 [out_dim][w], b3 [out_dim], flat in that order (torch's parameters() order).  Weights are in torch.nn.Linear
+ * layout ([out][in], fp32) with time as the LAST column of W0; x is [batch][dim], t [batch] (one time per row),
+ * target [batch][out_dim], row_scale [batch].  No input gradients.  grads may be null iff with_grad == 0; the loss has
+ * the same bits either way, and a call repeated on the same device gives the same bits (per-CTA partial sums folded
+ * in CTA order, no atomics).  supported(): w in {32, 64}, 1 <= dim <= 8, 1 <= out_dim <= 8, batch >= 1; rows stream
+ * from device memory, so the batch is not bounded by shared memory.  Argument errors are reported before any CUDA
+ * call. */
+int cfm_mlp_small_train_supported(int64_t batch, int dim, int w, int out_dim);
+size_t cfm_mlp_small_train_workspace_bytes(int64_t batch, int dim, int w, int out_dim);
+int cfm_mlp_small_mse_grad_f32(const float* W0, const float* b0, const float* W1, const float* b1,
+                               const float* W2, const float* b2, const float* W3, const float* b3,
+                               int dim, int w, int out_dim, int act, const float* x, const float* t,
+                               const float* target, const float* row_scale, int64_t batch, int with_grad,
+                               float* loss, float* grads, void* workspace, size_t workspace_bytes,
+                               void* stream);
+
 #ifdef __cplusplus
 }
 #endif
