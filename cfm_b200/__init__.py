@@ -19,6 +19,6 @@ from .models import MLP, SDE, GradModel, cnf_wrapper, torch_wrapper  # noqa: F40
 from .ode import NeuralODE  # noqa: F401
 from .optimal_transport import CouplingStream, OTPlanSampler, wasserstein  # noqa: F401
 from .sde import sdeint  # noqa: F401
-from .train import flow_matching_loss  # noqa: F401
+from .train import action_matching_loss, flow_matching_loss  # noqa: F401
 
 __version__ = "0.1.0"

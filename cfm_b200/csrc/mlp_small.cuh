@@ -33,6 +33,17 @@ __device__ __forceinline__ float act_deriv_fast(float x, int act) {
   return fmaf(x * s, 1.f - s, s);
 }
 
+// d^2 act / dx^2 at the pre-activation x, from the same ex2 approximation: SELU'' = lambda alpha e^x for x <= 0 and 0
+// for x > 0; SiLU'' = s (1 - s) (2 + x (1 - 2 s))
+__device__ __forceinline__ float act_deriv2_fast(float x, int act) {
+  if (act == CFM_ACT_SELU) {
+    const float negcoef = (float)(1.6732632423543772848170429916717 * 1.0507009873554804934193349852946);
+    return x > 0.f ? 0.f : ex2f(x * kLog2e) * negcoef;
+  }
+  const float s = __fdividef(1.f, 1.f + ex2f(-x * kLog2e));
+  return s * (1.f - s) * fmaf(x, fmaf(-2.f, s, 1.f), 2.f);
+}
+
 // acc[r][q] += sum_i m[i][u0 + q] * v[r][i] for the RB rows of v ([RB][W] in shared memory): m is [W][W] with the
 // lane's U columns contiguous, v is read as float4 broadcasts (the loop of mlp_eval's layers 1 and 2)
 template <int U>

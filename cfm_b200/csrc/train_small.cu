@@ -26,9 +26,7 @@
 //
 // with_grad = 0 stops each row after the loss and folds only the loss; the forward instructions are the same, so the
 // loss has the bits of the with-gradient call.
-#include <cooperative_groups.h>
-
-#include "mlp_small.cuh"
+#include "train_small.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -36,16 +34,7 @@ namespace cfm {
 
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
-constexpr int kTile = kWarps * RB;  // rows per CTA pass
-constexpr int kMaxDim = 8;          // dim and out_dim: layer 3 and the residual end in warp reductions
-constexpr int kInP = 16;            // floats per stashed input row: x, t, zero padding
-constexpr int kOutP = 8;            // floats per stashed delta_3 row
-// Most CTAs a launch uses and the workspace is sized for: one per SM of an H100 SXM (the launch also stays within the
-// device's own SMs).  Each CTA stages all weights and adds one partial-gradient vector to the fold, but on an H100
-// more CTAs were never slower, up to one per SM at every batch measured (DESIGN.md section 3.12).
-constexpr int kMaxCtas = 132;
+constexpr int kOutP = 8;  // floats per stashed delta_3 row
 
 struct TrainParams {
   const float *W0, *b0, *W1, *b1, *W2, *b2, *W3, *b3;  // torch Linear layout [out][in]; time = last column of W0
@@ -89,24 +78,6 @@ __host__ __device__ inline TrainPlan train_plan(int dim, int w, int out_dim) {
   s.red = take(2 * kWarps);
   s.total = o * sizeof(float);
   return s;
-}
-
-// parameters() order: W0 [w][dim + 1], b0, W1 [w][w], b1, W2, b2, W3 [out_dim][w], b3
-struct ParamOffsets {
-  int W0, b0, W1, b1, W2, b2, W3, b3, total;
-};
-__host__ __device__ inline ParamOffsets param_offsets(int dim, int w, int out_dim) {
-  ParamOffsets p;
-  p.W0 = 0;
-  p.b0 = p.W0 + w * (dim + 1);
-  p.W1 = p.b0 + w;
-  p.b1 = p.W1 + w * w;
-  p.W2 = p.b1 + w;
-  p.b2 = p.W2 + w * w;
-  p.W3 = p.b2 + w;
-  p.b3 = p.W3 + out_dim * w;
-  p.total = p.b3 + out_dim;
-  return p;
 }
 
 template <int U>
@@ -396,27 +367,10 @@ bool class_supported(int dim, int w, int out_dim) {
   return (w == 32 || w == 64) && dim >= 1 && dim <= kMaxDim && out_dim >= 1 && out_dim <= kMaxDim;
 }
 
-// CTAs a batch can use: one per tile of rows, up to kMaxCtas (the launch also stays within the device's SMs)
-int ctas_for(int64_t batch) {
-  const int64_t tiles = (batch + kTile - 1) / kTile;
-  return (int)(tiles < kMaxCtas ? tiles : kMaxCtas);
-}
-
 template <int U>
 int launch_train(TrainParams& p, int grid, char* ws, cudaStream_t s) {
-  const void* kern = (const void*)mlp_train_kernel<U>;
-  const size_t smem = train_plan(p.dim, 32 * U, p.out_dim).total;
-  CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 0;
-  CFM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-  CFM_REQUIRE(per_sm >= 1, "cfm_mlp_small_mse_grad_f32: the kernel does not fit on this device");
-  if (grid > per_sm * sm_count()) grid = per_sm * sm_count();  // a cooperative grid must be co-resident
-  p.loss_parts = reinterpret_cast<double*>(ws);
-  p.grad_parts = reinterpret_cast<float*>(ws + align_up((size_t)grid * sizeof(double), 256));
-  void* args[] = {&p};
-  CFM_CUDA_OK(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kThreads), args, smem, s));
-  note_launches(1);
-  return CFM_OK;
+  return launch_folded("cfm_mlp_small_mse_grad_f32", (const void*)mlp_train_kernel<U>,
+                       train_plan(p.dim, 32 * U, p.out_dim).total, p, grid, ws, s);
 }
 
 }  // namespace

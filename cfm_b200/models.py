@@ -179,7 +179,9 @@ class GradModel(torch.nn.Module):
     ``forward`` is plain PyTorch with ``create_graph=True``, so the action-matching loss backpropagates through it on
     any device; it needs autograd and fails under ``torch.no_grad()`` as the reference does.  Sampling
     ``torch_wrapper(GradModel(MLP(dim, out_dim=1, time_varying=True)))`` with ``cfm_b200.NeuralODE`` runs the forward
-    and reverse pass of the action in one kernel instead (csrc/ode_small.cu, gradient variant)."""
+    and reverse pass of the action in one kernel instead (csrc/ode_small.cu, gradient variant), and
+    ``cfm_b200.action_matching_loss(action, xt, t, x0, x1)`` computes the notebook's training loss and all parameter
+    gradients of such an action in one kernel (csrc/action_train.cu) without this double backward."""
 
     def __init__(self, action):
         super().__init__()

@@ -19,6 +19,10 @@ optimizer and DDP hooks work as with the eager lines.  The SF2M score loss
 Only the tutorial class of model is accelerated: ``cfm_b200.MLP(time_varying=True)`` with ``w`` in {32, 64},
 ``dim <= 8`` and ``out_dim <= 8``, fp32 on a CUDA device.  Anything else raises -- there is no eager fallback
 (``MLP.forward`` under autograd is still plain PyTorch for whoever wants it).  Gradients flow to the parameters only.
+
+``action_matching_loss(action, xt, t, x0, x1)`` does the same for the action-matching cell of the same notebook, whose
+loss needs a double backward: one kernel (csrc/action_train.cu) computes the loss, the input gradient of the action it
+contains, and all eight parameter gradients of ``MLP(dim, out_dim=1, time_varying=True)``.
 """
 import torch
 from torch.autograd.function import once_differentiable
@@ -43,13 +47,14 @@ def _launch(model, params, xt, t, ut, row_scale, with_grad):
     return loss, grads
 
 
-class _MseGrad(torch.autograd.Function):
-    """loss(parameters): forward computes the loss and, in the same launch, its gradients for upstream gradient 1;
-    backward scales that flat buffer by ``grad_output`` and hands out views of it."""
+class _FusedLossGrad(torch.autograd.Function):
+    """loss(parameters) of one library call ``launch(params, with_grad) -> (loss, flat gradients)``: forward computes the
+    loss and, in the same launch, its gradients for upstream gradient 1; backward scales that flat buffer by
+    ``grad_output`` and hands out views of it."""
 
     @staticmethod
-    def forward(ctx, model, xt, t, ut, row_scale, *params):
-        loss, grads = _launch(model, [p.detach().contiguous() for p in params], xt, t, ut, row_scale, True)
+    def forward(ctx, launch, *params):
+        loss, grads = launch([p.detach().contiguous() for p in params], True)
         ctx.grads = grads
         ctx.shapes = [p.shape for p in params]
         return loss
@@ -63,20 +68,54 @@ class _MseGrad(torch.autograd.Function):
             n = shape.numel()
             out.append(flat[o:o + n].view(shape))
             o += n
-        return (None, None, None, None, None, *out)
+        return (None, *out)
 
 
-def _check_model(model):
+def _attach(launch, params):
+    """The loss of ``launch`` on the parameters' autograd graph when autograd wants their gradients; else the loss only
+    (the kernel skips the gradients)."""
+    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+        return _FusedLossGrad.apply(launch, *params)
+    loss, _ = launch([p.detach().contiguous() for p in params], False)
+    return loss
+
+
+def _check_model(model, fn="flow_matching_loss", action=False):
+    out = "out_dim = 1" if action else "out_dim <= 8"
     if not isinstance(model, MLP):
         raise NotImplementedError(
-            f"flow_matching_loss: no training kernel for {type(model).__name__}; it takes "
-            "cfm_b200.MLP(time_varying=True) with w in {32, 64}, dim <= 8, out_dim <= 8")
-    if not (model.time_varying and model.w in (32, 64) and 1 <= model.dim <= 8 and 1 <= model.out_dim <= 8
+            f"{fn}: no training kernel for {type(model).__name__}; it takes "
+            f"cfm_b200.MLP(time_varying=True) with w in {{32, 64}}, dim <= 8, {out}")
+    if not (model.time_varying and model.w in (32, 64) and 1 <= model.dim <= 8
+            and (model.out_dim == 1 if action else 1 <= model.out_dim <= 8)
             and model.act in (_ffi.ACT_SELU, _ffi.ACT_SILU)):
         raise NotImplementedError(
-            f"flow_matching_loss: no training kernel for MLP(dim={model.dim}, out_dim={model.out_dim}, w={model.w}, "
+            f"{fn}: no training kernel for MLP(dim={model.dim}, out_dim={model.out_dim}, w={model.w}, "
             f"time_varying={model.time_varying}, act={model.act}); the kernel's class is w in {{32, 64}}, dim <= 8, "
-            "out_dim <= 8, time_varying=True, SELU or SiLU")
+            f"{out}, time_varying=True, SELU or SiLU")
+
+
+def _check_tensors(fn, tensors):
+    for name, v in tensors:
+        if not torch.is_tensor(v):
+            raise ValueError(f"{fn}: {name} must be a tensor; got {type(v).__name__}")
+        if v.requires_grad:
+            raise ValueError(f"{fn}: {name} requires grad, but gradients flow to the model's parameters "
+                             "only; detach it")
+
+
+def _check_devices(fn, model, tensors):
+    """The model's eight parameters, after checking that they and ``tensors`` are fp32 on one CUDA device."""
+    params = [p for lin in model._linears() for p in (lin.weight, lin.bias)]
+    dev = params[0].device
+    if dev.type != "cuda" or any(p.device != dev or p.dtype != torch.float32 for p in params):
+        raise _ffi.CfmLibraryError(f"{fn}: the MLP's parameters must be fp32 on one CUDA device (there "
+                                   "is no CPU fallback; the eager lines run anywhere)")
+    for name, v in tensors:
+        if v.device != dev or v.dtype != torch.float32:
+            raise _ffi.CfmLibraryError(f"{fn}: {name} must be fp32 on the parameters' device {dev}; got "
+                                       f"{v.dtype} on {v.device}")
+    return params
 
 
 def flow_matching_loss(model, xt, t, ut, row_scale=None):
@@ -88,12 +127,7 @@ def flow_matching_loss(model, xt, t, ut, row_scale=None):
     the loss); under ``torch.no_grad()`` the kernel computes the loss only, with the same bits."""
     _check_model(model)
     tensors = [("xt", xt), ("t", t), ("ut", ut)] + ([("row_scale", row_scale)] if row_scale is not None else [])
-    for name, v in tensors:
-        if not torch.is_tensor(v):
-            raise ValueError(f"flow_matching_loss: {name} must be a tensor; got {type(v).__name__}")
-        if v.requires_grad:
-            raise ValueError(f"flow_matching_loss: {name} requires grad, but gradients flow to the model's parameters "
-                             "only; detach it")
+    _check_tensors("flow_matching_loss", tensors)
     if xt.dim() != 2 or xt.shape[1] != model.dim or xt.shape[0] < 1:
         raise ValueError(f"flow_matching_loss: xt must be (B >= 1, {model.dim}); got {tuple(xt.shape)}")
     B = xt.shape[0]
@@ -103,19 +137,59 @@ def flow_matching_loss(model, xt, t, ut, row_scale=None):
         raise ValueError(f"flow_matching_loss: ut must be ({B}, {model.out_dim}); got {tuple(ut.shape)}")
     if row_scale is not None and tuple(row_scale.shape) != (B,):
         raise ValueError(f"flow_matching_loss: row_scale must be ({B},); got {tuple(row_scale.shape)}")
-    params = [p for lin in model._linears() for p in (lin.weight, lin.bias)]
-    dev = params[0].device
-    if dev.type != "cuda" or any(p.device != dev or p.dtype != torch.float32 for p in params):
-        raise _ffi.CfmLibraryError("flow_matching_loss: the MLP's parameters must be fp32 on one CUDA device (there "
-                                   "is no CPU fallback; the eager lines run anywhere)")
-    for name, v in tensors:
-        if v.device != dev or v.dtype != torch.float32:
-            raise _ffi.CfmLibraryError(f"flow_matching_loss: {name} must be fp32 on the parameters' device {dev}; got "
-                                       f"{v.dtype} on {v.device}")
+    params = _check_devices("flow_matching_loss", model, tensors)
     xt, t, ut = xt.contiguous(), t.contiguous(), ut.contiguous()
     if row_scale is not None:
         row_scale = row_scale.contiguous()
-    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
-        return _MseGrad.apply(model, xt, t, ut, row_scale, *params)
-    loss, _ = _launch(model, [p.detach().contiguous() for p in params], xt, t, ut, row_scale, False)
-    return loss
+    return _attach(lambda ps, with_grad: _launch(model, ps, xt, t, ut, row_scale, with_grad), params)
+
+
+def _launch_action(model, params, xt, t, x0, x1, with_grad):
+    """One library call: (loss 0-d, flat gradient buffer in parameters() order or None)."""
+    L = _ffi.lib()
+    dev = xt.device
+    B = xt.shape[0]
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    grads = torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev) if with_grad else None
+    ws = _ffi.workspace(L.cfm_mlp_small_train_workspace_bytes(B, model.dim, model.w, 1), dev)
+    with torch.cuda.device(dev):  # kernels launch on the current device: make it the tensors' one
+        _ffi.check(L.cfm_mlp_small_action_grad_f32(
+            *[_ffi.ptr(p) for p in params], model.dim, model.w, model.act, _ffi.ptr(xt), _ffi.ptr(t), _ffi.ptr(x0),
+            _ffi.ptr(x1), B, 1 if with_grad else 0, _ffi.ptr(loss), _ffi.ptr(grads), _ffi.ptr(ws), ws.numel(),
+            _ffi.stream_ptr(dev)), "cfm_mlp_small_action_grad_f32")
+    return loss, grads
+
+
+def action_matching_loss(action, xt, t, x0, x1):
+    """The action-matching loss of tutorial_training_8_gaussians_to_moons.ipynb (cell 11) as a 0-d fp32 CUDA tensor:
+
+        mean_r [ s(x0_r, 0) - s(x1_r, 1) + 1/2 |d s / d x (xt_r, t_r)|^2 + d s / d t (xt_r, t_r) ]
+
+    for the scalar action ``s = action``, a ``cfm_b200.MLP(dim, out_dim=1, w, time_varying=True)`` with ``w`` in
+    {32, 64}, ``dim <= 8``, SELU or SiLU.  It replaces the notebook's double backward:
+
+        st = torch.sum(action(torch.cat([xt, t], dim=-1)))
+        dsdx, dsdt = torch.autograd.grad(st, (xt, t), create_graph=True, retain_graph=True)
+        a0 = action(torch.cat([x0, torch.zeros(batch_size, 1)], dim=-1))
+        a1 = action(torch.cat([x1, torch.ones(batch_size, 1)], dim=-1))
+        loss = (a0 - a1 + 0.5 * (dsdx**2).sum(1, keepdims=True) + dsdt).mean()
+
+    ``xt``, ``x0``, ``x1`` (B, dim) and ``t`` (B,) or (B, 1): fp32 on the parameters' CUDA device, not requiring grad.
+    With autograd enabled the result carries the gradients of the action's eight parameters, computed in the same
+    launch as the loss (``b3``'s is exactly 0); under ``torch.no_grad()`` the kernel computes the loss only, with the
+    same bits."""
+    fn = "action_matching_loss"
+    _check_model(action, fn, action=True)
+    tensors = [("xt", xt), ("t", t), ("x0", x0), ("x1", x1)]
+    _check_tensors(fn, tensors)
+    if xt.dim() != 2 or xt.shape[1] != action.dim or xt.shape[0] < 1:
+        raise ValueError(f"{fn}: xt must be (B >= 1, {action.dim}); got {tuple(xt.shape)}")
+    B = xt.shape[0]
+    if tuple(t.shape) not in ((B,), (B, 1)):
+        raise ValueError(f"{fn}: t must be ({B},) or ({B}, 1), one time per row; got {tuple(t.shape)}")
+    for name, v in (("x0", x0), ("x1", x1)):
+        if tuple(v.shape) != (B, action.dim):
+            raise ValueError(f"{fn}: {name} must be ({B}, {action.dim}); got {tuple(v.shape)}")
+    params = _check_devices(fn, action, tensors)
+    xt, t, x0, x1 = xt.contiguous(), t.reshape(B).contiguous(), x0.contiguous(), x1.contiguous()
+    return _attach(lambda ps, with_grad: _launch_action(action, ps, xt, t, x0, x1, with_grad), params)

@@ -374,6 +374,21 @@ int cfm_mlp_small_mse_grad_f32(const float* W0, const float* b0, const float* W1
                                float* loss, float* grads, void* workspace, size_t workspace_bytes,
                                void* stream);
 
+/* The action-matching loss of the 2-D tutorial (tutorial_training_8_gaussians_to_moons.ipynb, cell 11), which the
+ * notebook differentiates with a double backward:
+ *     loss = mean_r [ s(x0_r, 0) - s(x1_r, 1) + 1/2 sum_{d < dim} (d s / d x_d)(xt_r, t_r)^2 + (d s / d t)(xt_r, t_r) ]
+ * for the scalar action s = MLP(dim, out_dim=1, w, time_varying=True).  When with_grad != 0, d loss / d parameter goes
+ * to grads in the layout of cfm_mlp_small_mse_grad_f32 with out_dim = 1; the gradient of b3 is exactly 0 (b3 cancels
+ * in s(x0) - s(x1) and does not enter grad s).  xt, x0, x1 are [batch][dim], t [batch].  The workspace is sized by
+ * cfm_mlp_small_train_workspace_bytes(batch, dim, w, 1).  grads may be null iff with_grad == 0; the loss has the same
+ * bits either way, and a call repeated on the same device gives the same bits.  Supported: w in {32, 64},
+ * 1 <= dim <= 8, batch >= 1, SELU or SiLU.  Argument errors are reported before any CUDA call. */
+int cfm_mlp_small_action_grad_f32(const float* W0, const float* b0, const float* W1, const float* b1,
+                                  const float* W2, const float* b2, const float* W3, const float* b3,
+                                  int dim, int w, int act, const float* xt, const float* t, const float* x0,
+                                  const float* x1, int64_t batch, int with_grad, float* loss, float* grads,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
