@@ -13,6 +13,8 @@
   numerics/solvers/ode.py::DormandPrince45, numerics/utils.py::{hairer_norm,
   init_step,adapt_step}; SURVEY.md Appendix B).  PARITY UNPINNED: the reference
   holds no numeric test of any trajectory (tests/test_models.py only constructs).
+  ``record=[]`` collects one entry per step attempt (t, dt, ratio, accepted,
+  clipped), for tests that must know which controller branches a case takes.
 """
 import torch
 
@@ -121,10 +123,15 @@ def dopri5_step(f, x, t, dt, k1):
 
 
 @torch.no_grad()
-def dopri5_trajectory(f, x, t_span, atol=1e-4, rtol=1e-4):
+def dopri5_trajectory(f, x, t_span, atol=1e-4, rtol=1e-4, record=None):
     """torchdyn odeint(..., solver='dopri5') without interpolator: adaptive
     lock-step over the batch, ONE scalar step size (global RMS error norm), every
-    t_span entry hit exactly by clipping dt.  Returns (traj, stats)."""
+    t_span entry hit exactly by clipping dt.  Returns (traj, stats).
+
+    ``record``: an optional list; every step attempt appends a dict with the ``t`` it
+    started from, the ``dt`` it took (after clipping), its error ``ratio``, whether it
+    was ``accepted`` and whether it was ``clipped`` onto a checkpoint (``ckpt_flag``).
+    The integration itself does not depend on it."""
     t_span = t_span.to(x)
     t, T = t_span[0], t_span[-1]
     k1 = f(t, x)
@@ -148,6 +155,9 @@ def dopri5_trajectory(f, x, t_span, atol=1e-4, rtol=1e-4):
         tol = atol + rtol * torch.max(x.abs(), x_new.abs())
         ratio = hairer_norm(err / tol)
         accept = bool(ratio <= 1)
+        if record is not None:
+            record.append({"t": float(t), "dt": float(dt), "ratio": float(ratio), "accepted": accept,
+                           "clipped": ckpt_flag})
         if accept:
             if ckpt < len(t_span) and t + dt == t_span[ckpt]:
                 sol.append(x_new)

@@ -36,11 +36,12 @@ def _reversed(f):
     return lambda s, z: -f(-s, z)
 
 
-def dopri5_any_direction(f, x, t_span, atol=1e-4, rtol=1e-4):
-    """(traj, stats) of torchdyn's dopri5 over ``t_span`` in either direction."""
+def dopri5_any_direction(f, x, t_span, atol=1e-4, rtol=1e-4, record=None):
+    """(traj, stats) of torchdyn's dopri5 over ``t_span`` in either direction.  ``record``: see
+    ``oracle.vector_field.dopri5_trajectory``; for a decreasing span its times are those of the reversed run, -t."""
     if t_span[1] < t_span[0]:
-        return vf.dopri5_trajectory(_reversed(f), x, -t_span, atol, rtol)
-    return vf.dopri5_trajectory(f, x, t_span, atol, rtol)
+        return vf.dopri5_trajectory(_reversed(f), x, -t_span, atol, rtol, record=record)
+    return vf.dopri5_trajectory(f, x, t_span, atol, rtol, record=record)
 
 
 def euler_any_direction(f, x, t_span):

@@ -7,7 +7,8 @@
 * Plain variant: one test per compiled ode_small_kernel<U, MAXT, false>, with the profiler naming the kernel that
   ran.  A CPU test reads the instantiations out of the built library, so a new one without a test fails there.
 * MLP: the per-layer fp16x3 tensor-core path (and the SIMT path) at hidden widths that are not multiples of 32, one
-  partial K-chunk, and w = 512; the multi-kernel dopri5 driver on it.
+  partial K-chunk, and w = 512; the multi-kernel dopri5 driver on it (that driver's own tests, path by path and
+  kernel by kernel, are in tests/test_gpu_dopri5_driver.py).
 
 Batch sizes follow from the device's SM count or from the library's own plan queries, so the cases keep their meaning
 on a part with a different SM count."""
