@@ -11,6 +11,8 @@
 //   * (algo 2) row-scaled fp16 (hi, lo) splits of all weights for the tensor-core paths (mlp_h3.cu).
 // algo 1 (this file): four SIMT fp32 GEMMs with fused bias + activation epilogues (true fp32
 // FMA, the numerics of the reference's cuBLAS sgemm with TF32 off).
+// algo 2: the tensor-core paths (mlp_h3.cu).  They need a shape mlp_tc_supported() accepts AND 16-byte aligned
+// x, y and workspace; algo 0 takes them when both hold and the SIMT path otherwise.
 #include "gemm_simt.cuh"
 #include "mlp_common.cuh"
 
@@ -115,7 +117,11 @@ extern "C" int cfm_mlp_forward_f32(const void* prepared, const float* x, int bat
   const MlpBlobHeader h = mlp_layout(dim, w, out_dim, time_varying ? 1 : 0);
   const bool tc_ok = mlp_tc_supported(batch, dim, w, out_dim) != 0;
   if (algo == 2) CFM_REQUIRE(tc_ok, "cfm_mlp_forward_f32: tensor-core path unsupported for this shape");
-  const bool use_tc = algo == 2 || (algo == 0 && tc_ok);
+  // the tensor-core path also needs 16-byte aligned x, y and workspace (TMA maps, vector stores); auto mode sends any
+  // other pointers to the SIMT path, which takes every alignment, and algo 2 refuses them in mlp_tc_forward
+  const bool tc_aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) |
+                            reinterpret_cast<uintptr_t>(workspace)) & 15) == 0;
+  const bool use_tc = algo == 2 || (algo == 0 && tc_ok && tc_aligned);
   CFM_REQUIRE(workspace_bytes >= cfm_mlp_workspace_bytes(batch, dim, w, out_dim, use_tc ? 2 : 1),
               "cfm_mlp_forward_f32: workspace too small");
   const char* B = reinterpret_cast<const char*>(prepared);

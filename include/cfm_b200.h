@@ -199,6 +199,9 @@ int cfm_flow_pairs_f32(int kind, const float* x0, const float* x1, const int64_t
  * *t_dev (device float) when t_dev != NULL, else t_host is used.
  * prepared: opaque device blob built once per weight set by cfm_mlp_prepare (split /
  * padded copies of the weights); workspace holds the two hidden activations.
+ * algo: 0 auto (the tensor-core paths when cfm_mlp_tc_supported() accepts the shape and x, y and
+ * the workspace are 16-byte aligned, SIMT fp32 otherwise), 1 SIMT fp32, 2 tensor cores (fails on a
+ * shape or a pointer they cannot take).
  */
 size_t cfm_mlp_prepared_bytes(int dim, int w, int out_dim, int time_varying);
 int cfm_mlp_prepare(const float* W0, const float* b0, const float* W1, const float* b1,

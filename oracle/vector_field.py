@@ -38,15 +38,17 @@ def make_mlp(dim, out_dim=None, w=64, time_varying=False, dtype=torch.float32):
     return _MLP().to(dtype)
 
 
-def mlp_forward_from_state(state, x, dtype=torch.float64):
-    """models.py:20-21 evaluated from a state_dict in ``dtype`` (float64 gate)."""
+def mlp_forward_from_state(state, x, dtype=torch.float64, act="selu"):
+    """models.py:20-21 evaluated from a state_dict in ``dtype`` (float64 gate), on the device of ``x``.
+    ``act="silu"``: the SiLU variant of the MLP (the library's ACT_SILU)."""
+    f = {"selu": torch.nn.functional.selu, "silu": torch.nn.functional.silu}[act]
     h = x.to(dtype)
     for li in (0, 2, 4, 6):
-        W = state[f"net.{li}.weight"].to(dtype)
-        b = state[f"net.{li}.bias"].to(dtype)
+        W = state[f"net.{li}.weight"].to(device=h.device, dtype=dtype)
+        b = state[f"net.{li}.bias"].to(device=h.device, dtype=dtype)
         h = h @ W.T + b
         if li != 6:
-            h = torch.nn.functional.selu(h)
+            h = f(h)
     return h
 
 
