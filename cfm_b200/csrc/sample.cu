@@ -9,7 +9,7 @@
 //      entries recomputed from (M, log_u, log_v) to find the column where the cdf crosses.
 // This equals the flat searchsorted up to float64 rounding of the cumulative sums.  The uniforms
 // come from the host's np.random stream so the reference's RNG contract is kept.
-#include "common.cuh"
+#include "sinkhorn_common.cuh"
 
 namespace cfm {
 
@@ -345,8 +345,8 @@ __global__ void draw_uniform_rows_kernel(const float* __restrict__ M, int n0, in
   const float c2 = -kLog2e / (reg * scale);
   const float* row = M + (int64_t)i * ldm;
   const bool vec = ((ldm & 3) == 0) && ((n1 & 3) == 0) && ((reinterpret_cast<uintptr_t>(M) & 15) == 0);
-  // same rule as the solver's auto mode: beyond |M/reg| ~ 64 the exponent needs float64 adds
-  const bool precise = cost_max ? !((normalize ? 1.f : cmax) / reg <= 64.f) : true;
+  // the solver's auto-mode rule: beyond |M/reg| ~ 64 the exponent needs float64 adds
+  const bool precise = cost_max ? sk_needs_f64(cmax, normalize, reg) : true;
   int jsel;
   // with log_u the weights are pi_ij and their row sum is a_i = 1/n0 (row update last): no totalling pass.  A
   // potential pair that is not finite (NaN costs) falls back to the measured total, which flags it.  So does a solve

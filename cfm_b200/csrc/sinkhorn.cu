@@ -153,6 +153,124 @@ __device__ __forceinline__ double row_lse_screened(const float* __restrict__ row
 }
 
 
+// ---- pieces of the column phase and the combine, shared by both solver bodies ---------------------------------
+// float4 group g of the 8 rows r0 .. r0 + 7 of M; rows at or past R, and every row when !valid, are +inf (zero
+// weight).  L1: plain __ldg for an aligned row block the caller has just read (seeded fused sweep), else load_cost4.
+template <bool VEC, bool L1 = false>
+__device__ __forceinline__ void load_block8(float4 (&c)[8], const SkParams& p, int r0, int R, int g, bool valid) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    if (valid && q < R) {
+      const float* row = p.M + (int64_t)(r0 + q) * p.ldm;
+      c[q] = (VEC && L1) ? __ldg(reinterpret_cast<const float4*>(row + g * 4)) : load_cost4<VEC>(row, g * 4, p.n1);
+    } else {
+      const float inf = __int_as_float(0x7f800000);
+      c[q] = make_float4(inf, inf, inf, inf);
+    }
+  }
+}
+
+// row e < 8 of a register block (three levels of selects, no reload)
+__device__ __forceinline__ float4 pick8(const float4 (&c)[8], int e) {
+  const float4 c01 = (e & 1) ? ((e & 2) ? c[3] : c[1]) : ((e & 2) ? c[2] : c[0]);
+  const float4 c45 = (e & 1) ? ((e & 2) ? c[7] : c[5]) : ((e & 2) ? c[6] : c[4]);
+  return (e & 4) ? c45 : c01;
+}
+
+// this CTA's column partials of the thread's float4 groups g = g0 + tid + 512 k
+template <int KG, class PT, class ST>
+__device__ __forceinline__ void store_partials(const SkParams& p, const PT (&cm)[KG][4], const ST (&cs)[KG][4],
+                                               int g0) {
+  const int ng = p.n1p / 4;
+#pragma unroll
+  for (int k = 0; k < KG; ++k) {
+    const int g = g0 + threadIdx.x + kSkThreads * k;
+    if (g >= ng) continue;
+    PT* pm = reinterpret_cast<PT*>(p.part_m) + (int64_t)blockIdx.x * p.n1p + g * 4;
+    ST* ps = reinterpret_cast<ST*>(p.part_s) + (int64_t)blockIdx.x * p.n1p + g * 4;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) { pm[c] = cm[k][c]; ps[c] = cs[k][c]; }
+  }
+}
+
+// v_cur -> shared memory (padding 0) and, when vh_s is not null, its fp32 copy for the screening
+template <class T>
+__device__ __forceinline__ void stage_v(T* v_s, float* vh_s, const T* v_cur, int n1, int n1p) {
+  for (int j = threadIdx.x; j < n1p; j += kSkThreads) {
+    const T vj = (j < n1) ? __ldcg(v_cur + j) : (T)0;
+    v_s[j] = vj;
+    if (vh_s != nullptr) vh_s[j] = (float)vj;
+  }
+  __syncthreads();
+}
+
+// Combine the per-CTA column partials of this CTA's slice of columns: v_new = logb - LSE over the CTAs (8 lanes per
+// column).  With v_cur (not null) the squared column-marginal error of (u, v_cur) goes to *err_slot, and the return
+// value is the thread's minimum of v_new - v_cur (3e38 otherwise).  Ends with a block barrier only when it sums.
+template <bool P, bool MIX>
+__device__ __forceinline__ float combine_cols(const SkParams& p, const typename Tr<P>::pot_t* v_cur,
+                                              typename Tr<P>::pot_t* v_new, typename Tr<P>::pot_t logb, double to_ln,
+                                              double* err_slot, double* red) {
+  using pot_t = typename Tr<P>::pot_t;
+  using sum_t = typename Tr<P>::sum_t;
+  const pot_t* part_m = reinterpret_cast<const pot_t*>(p.part_m);
+  const sum_t* part_s = reinterpret_cast<const sum_t*>(p.part_s);
+  const int tid = threadIdx.x, nblk = gridDim.x, n1 = p.n1, n1p = p.n1p;
+  const int cpc = (n1 + nblk - 1) / nblk;
+  const int c_begin = blockIdx.x * cpc, c_end = min(n1, c_begin + cpc);
+  double err_local = 0.0;
+  float dmin = 3.0e38f;
+  const int sub = tid & 7;
+  for (int j0 = c_begin; j0 < c_end; j0 += (kSkThreads >> 3)) {
+    // every thread takes the same trip count (shuffles below); idle columns contribute nothing
+    const int j = j0 + (tid >> 3);
+    const bool act = j < c_end;
+    pot_t m = Tr<P>::init();
+    sum_t s = 0;
+    if (act) {
+      for (int c0 = sub; c0 < nblk; c0 += 8 * 4) {
+        pot_t mm[4];
+        sum_t ss[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int c = c0 + q * 8;
+          if (c < nblk) {
+            mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
+            ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
+          } else { mm[q] = Tr<P>::init(); ss[q] = 0; }
+        }
+        pot_t bm = vmax(vmax(mm[0], mm[1]), vmax(mm[2], mm[3]));
+        bm = vmax(bm, m);
+        sum_t acc = s * expd<MIX>(m, bm);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc += ss[q] * expd<MIX>(mm[q], bm);
+        s = acc; m = bm;
+      }
+    }
+    // reduce over the 8 lanes of this column
+    pot_t gm = m;
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) gm = vmax(gm, __shfl_xor_sync(0xffffffffu, gm, o));
+    sum_t gs = s * expd<MIX>(m, gm);
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);
+    if (act && sub == 0) {
+      const pot_t vn = logb - lse_fin(gm, gs);
+      v_new[j] = vn;
+      if (v_cur != nullptr) {
+        // column marginal of (u, v_cur): exp(v_cur + lse); POT: err = ||colsum - b||_2
+        const pot_t vc = __ldcg(v_cur + j);
+        dmin = fminf(dmin, __double2float_rd((double)vn - (double)vc));
+        const double e = expm1(((double)vc - (double)vn) * to_ln) / (double)n1;
+        err_local += e * e;
+      }
+    }
+  }
+  if (v_cur != nullptr) sk_err_add(err_local, err_slot, red);
+  return dmin;
+}
+
+
 // ---- the solver body ---------------------------------------------------------------------------
 template <bool P, bool VEC, int KG, bool MIX>
 __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
@@ -160,7 +278,6 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
   using sum_t = typename Tr<P>::sum_t;
   cg::grid_group grid = cg::this_grid();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int nblk = gridDim.x, b = blockIdx.x;
   const int n0 = p.n0, n1 = p.n1, n1p = p.n1p, ng = n1p / 4;
 
   __shared__ pot_t u_chunk[kSkChunk];
@@ -175,8 +292,6 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
 
   pot_t* u_work = reinterpret_cast<pot_t*>(p.u_work);
   pot_t* v_work[2] = {reinterpret_cast<pot_t*>(p.v_work[0]), reinterpret_cast<pot_t*>(p.v_work[1])};
-  pot_t* part_m = reinterpret_cast<pot_t*>(p.part_m);
-  sum_t* part_s = reinterpret_cast<sum_t*>(p.part_s);
 
   // element transform and the log-marginals in this mode's units
   Xf<P> xf;
@@ -193,22 +308,13 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
   const double to_ln = P ? 1.0 : kLn2d;  // working units -> natural log
   const float nr = -1.f / (p.reg * (p.normalize ? cmax : 1.f));  // screening only: t ~ -M/(reg scale) + potential
 
-  // slab of rows owned by this CTA (first `rem` CTAs get one extra row)
-  const int base = n0 / nblk, rem = n0 % nblk;
-  const int r_begin = b * base + min(b, rem);
-  const int r_end = r_begin + base + (b < rem ? 1 : 0);
+  const SkSlab slab = sk_slab(n0, gridDim.x, blockIdx.x);
+  const int r_begin = slab.begin, r_end = slab.end;
   const int npanel = (n1p + kPanelCols - 1) / kPanelCols;
 
   // one sweep: (optional) row phase -> u ; (optional) column partials with that u
   auto sweep = [&](bool do_row, bool do_col, const pot_t* v_cur) {
-    if (do_row && p.v_in_smem) {
-      for (int j = tid; j < n1p; j += kSkThreads) {
-        const pot_t vj = (j < n1) ? __ldcg(v_cur + j) : (pot_t)0;
-        v_s[j] = vj;
-        if (screen) vh_s[j] = (float)vj;
-      }
-      __syncthreads();
-    }
+    if (do_row && p.v_in_smem) stage_v(v_s, screen ? vh_s : nullptr, v_cur, n1, n1p);
     const pot_t* vsrc = p.v_in_smem ? v_s : v_cur;
     for (int panel = 0; panel < npanel; ++panel) {
       pot_t cm[KG][4];
@@ -256,18 +362,9 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
 #pragma unroll
             for (int k = 0; k < KG; ++k) {
               const int g = gpan + tid + kSkThreads * k;
-              const bool gv = g < ng;
               for (int rb = 0; rb < R; rb += 8) {
                 float4 c[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  if (gv && rb + q < R) {
-                    c[q] = load_cost4<VEC>(p.M + (int64_t)(r0 + rb + q) * p.ldm, g * 4, n1);
-                  } else {
-                    const float inf = __int_as_float(0x7f800000);
-                    c[q] = make_float4(inf, inf, inf, inf);
-                  }
-                }
+                load_block8<VEC>(c, p, r0 + rb, R - rb, g, g < ng);
                 float uh[8];
 #pragma unroll
                 for (int q = 0; q < 8; ++q) uh[q] = uh_chunk[(rb + q) & (kSkChunk - 1)];
@@ -291,10 +388,7 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
                     if (mask != 0u) {
                       const int e = __ffs((int)mask) - 1;
                       mask &= mask - 1u;
-                      // the cost entry of row e out of registers (three levels of selects, no reload)
-                      const float4 c01 = (e & 1) ? ((e & 2) ? c[3] : c[1]) : ((e & 2) ? c[2] : c[0]);
-                      const float4 c45 = (e & 1) ? ((e & 2) ? c[7] : c[5]) : ((e & 2) ? c[6] : c[4]);
-                      const float4 ce = (e & 4) ? c45 : c01;
+                      const float4 ce = pick8(c, e);
                       const float cv = cc == 0 ? ce.x : cc == 1 ? ce.y : cc == 2 ? ce.z : ce.w;
                       lse_take(xf(cv, u_chunk[(rb + e) & (kSkChunk - 1)]), cm[k][cc], cs[k][cc]);
                     }
@@ -312,15 +406,7 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
           if (g >= ng) continue;
           for (int rb = 0; rb < R; rb += 8) {
             float4 c[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              if (rb + q < R) {
-                c[q] = load_cost4<VEC>(p.M + (int64_t)(r0 + rb + q) * p.ldm, g * 4, n1);
-              } else {
-                const float inf = __int_as_float(0x7f800000);
-                c[q] = make_float4(inf, inf, inf, inf);
-              }
-            }
+            load_block8<VEC>(c, p, r0 + rb, R - rb, g, true);
 #pragma unroll
             for (int cc = 0; cc < 4; ++cc) {
               pot_t x[8];
@@ -341,130 +427,33 @@ __device__ void sinkhorn_run(const SkParams& p, unsigned char* smem_raw) {
         }
         __syncthreads();  // u_chunk is rewritten by the next chunk's row phase
       }
-      if (do_col) {
-#pragma unroll
-        for (int k = 0; k < KG; ++k) {
-          const int g = gpan + tid + kSkThreads * k;
-          if (g >= ng) continue;
-          pot_t* pm = part_m + (int64_t)b * n1p + g * 4;
-          sum_t* ps = part_s + (int64_t)b * n1p + g * 4;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) { pm[c] = cm[k][c]; ps[c] = cs[k][c]; }
-        }
-      }
-    }
-  };
-
-  // combine the per-CTA column partials of a slice of columns -> v_new, marginal error
-  auto combine = [&](const pot_t* v_cur, pot_t* v_new, bool have_cur, double* err_slot) {
-    const int cpc = (n1 + nblk - 1) / nblk;
-    const int c_begin = b * cpc, c_end = min(n1, c_begin + cpc);
-    double err_local = 0.0;
-    const int sub = tid & 7;
-    for (int j0 = c_begin; j0 < c_end; j0 += (kSkThreads >> 3)) {
-      // every thread takes the same trip count (shuffles below); idle columns contribute nothing
-      const int j = j0 + (tid >> 3);
-      const bool act = j < c_end;
-      pot_t m = Tr<P>::init();
-      sum_t s = 0;
-      if (act) {
-        for (int c0 = sub; c0 < nblk; c0 += 8 * 4) {
-          pot_t mm[4];
-          sum_t ss[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int c = c0 + q * 8;
-            if (c < nblk) {
-              mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
-              ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
-            } else { mm[q] = Tr<P>::init(); ss[q] = 0; }
-          }
-          pot_t bm = vmax(vmax(mm[0], mm[1]), vmax(mm[2], mm[3]));
-          bm = vmax(bm, m);
-          sum_t acc = s * expd<MIX>(m, bm);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc += ss[q] * expd<MIX>(mm[q], bm);
-          s = acc; m = bm;
-        }
-      }
-      // reduce over the 8 lanes of this column
-      pot_t gm = m;
-#pragma unroll
-      for (int o = 4; o > 0; o >>= 1) gm = vmax(gm, __shfl_xor_sync(0xffffffffu, gm, o));
-      sum_t gs = s * expd<MIX>(m, gm);
-#pragma unroll
-      for (int o = 4; o > 0; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);
-      if (act && sub == 0) {
-        const pot_t lse = lse_fin(gm, gs);
-        const pot_t vn = logb - lse;
-        v_new[j] = vn;
-        if (have_cur) {
-          // column marginal of (u, v_cur): exp(v_cur + lse); POT: err = ||colsum - b||_2
-          const double d = ((double)__ldcg(v_cur + j) - (double)vn) * to_ln;
-          const double e = expm1(d) / (double)n1;
-          err_local += e * e;
-        }
-      }
-    }
-    if (err_slot != nullptr) {
-      err_local = warp_sum(err_local);
-      if (lane == 0) red[warp] = err_local;
-      __syncthreads();
-      if (warp == 0) {
-        double t = lane < kSkWarps ? red[lane] : 0.0;
-        t = warp_sum(t);
-        if (lane == 0) atomicAdd(err_slot, t);
-      }
-      __syncthreads();
+      if (do_col) store_partials<KG>(p, cm, cs, gpan);
     }
   };
 
   // ---- prologue: v^0 = logb - LSE_i(Mr_ij + 0) ----
-  if (b == 0 && tid < 4) p.err_ring[tid] = 0.0;
+  sk_ring_init(p);
   sweep(false, true, nullptr);
   grid.sync();
-  combine(nullptr, v_work[0], false, nullptr);
+  combine_cols<P, MIX>(p, nullptr, v_work[0], logb, to_ln, nullptr, red);
   grid.sync();
 
-  int cur = 0, iters = 0;
-  bool converged = false;
-  double err = 1.0, prev_check_err = -1.0;
+  SkLoop L;
+  int cur = 0;
   for (int it = 0; it < p.max_iters; ++it) {
-    const bool last = (it == p.max_iters - 1);
-    const bool check = (it % p.check_every) == 0;
-    const bool do_col = !last || check;
-    sweep(true, do_col, v_work[cur]);
-    iters = it + 1;
-    if (!do_col) break;
+    const SkStep st = sk_step(p, it);
+    sweep(true, st.do_col, v_work[cur]);
+    L.iters = it + 1;
+    if (!st.do_col) break;
     grid.sync();
-    if (b == 0 && tid == 0) p.err_ring[(it + 2) & 3] = 0.0;
-    combine(v_work[cur], v_work[cur ^ 1], true, &p.err_ring[it & 3]);
+    double* err_slot = sk_err_slot(p, it);
+    combine_cols<P, MIX>(p, st.check ? v_work[cur] : nullptr, v_work[cur ^ 1], logb, to_ln, err_slot, red);
     grid.sync();
-    if (check) {
-      err = sqrt(__ldcg(&p.err_ring[it & 3]));
-      if (err < p.stop_thr) { converged = true; break; }
-      if (p.stall_tol > 0.0 && prev_check_err >= 0.0 &&
-          err > (1.0 - p.stall_tol) * prev_check_err &&
-          err * sqrt((double)n1) < 1e-5) { converged = true; break; }
-      prev_check_err = err;
-    }
-    if (last) break;
+    if (st.check && sk_check_stops(L, p, it)) break;
+    if (st.last) break;
     cur ^= 1;
   }
-
-  // ---- outputs ----
-  for (int j = b * kSkThreads + tid; j < n1; j += nblk * kSkThreads)
-    p.log_v[j] = (double)__ldcg(v_work[cur] + j) * to_ln;
-  if (b == 0 && tid == 0) {
-    int flags = 0;
-    if (!converged) flags |= CFM_FLAG_NOT_CONVERGED;
-    if (!(err == err)) flags |= CFM_FLAG_NONFINITE;
-    p.status[0] = flags;
-    p.status[1] = iters;
-    p.status[2] = P ? (MIX ? 2 : 1) : 0;  // 0 fp32, 1 float64, 2 float64 arguments + fp32 exponentials
-    p.status[3] = 0;
-    *p.err_out = err;
-  }
+  sk_finish(p, L, v_work[cur], to_ln, P ? (MIX ? 2 : 1) : 0, 0);
 }
 
 
@@ -532,6 +521,37 @@ __device__ __forceinline__ double row_lse_seeded(const float* __restrict__ row, 
   return lse_fin(wm, ws);
 }
 
+// seeded column pass over one block of 8 rows (u of row q in u_s[q], its fp32 copy in uh_s[q]) and the thread's four
+// columns: the rows with a term above the column's threshold are the candidates; their terms above it take the
+// exact path
+__device__ __forceinline__ void col_block_seeded(const float4 (&c)[8], const double* u_s, const float* uh_s,
+                                                 const float (&thr)[4], double (&cm)[4], double (&cs)[4],
+                                                 const Xf<true>& xf, float nr) {
+  float uh[8];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) uh[q] = uh_s[q];
+  unsigned hm = 0;  // bit q: row q of the block holds a candidate in one of the four columns
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const bool le = (fmaf(c[q].x, nr, uh[q]) <= thr[0]) & (fmaf(c[q].y, nr, uh[q]) <= thr[1]) &
+                    (fmaf(c[q].z, nr, uh[q]) <= thr[2]) & (fmaf(c[q].w, nr, uh[q]) <= thr[3]);
+    hm |= (le ? 0u : 1u) << q;
+  }
+  while (__any_sync(0xffffffffu, hm != 0u)) {
+    if (hm != 0u) {
+      const int e = __ffs((int)hm) - 1;
+      hm &= hm - 1u;
+      const float4 ce = pick8(c, e);
+      const float ue = uh_s[e];
+      const double ud = u_s[e];
+      if (!(fmaf(ce.x, nr, ue) <= thr[0])) lse_take(xf(ce.x, ud), cm[0], cs[0]);
+      if (!(fmaf(ce.y, nr, ue) <= thr[1])) lse_take(xf(ce.y, ud), cm[1], cs[1]);
+      if (!(fmaf(ce.z, nr, ue) <= thr[2])) lse_take(xf(ce.z, ud), cm[2], cs[2]);
+      if (!(fmaf(ce.w, nr, ue) <= thr[3])) lse_take(xf(ce.w, ud), cm[3], cs[3]);
+    }
+  }
+}
+
 __device__ __forceinline__ float block_min_f(float v, float* red32, int tid) {
   v = -warp_max(-v);
   if ((tid & 31) == 0) red32[tid >> 5] = v;
@@ -561,10 +581,6 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
 
   double* u_work = reinterpret_cast<double*>(p.u_work);
   double* v_work[2] = {reinterpret_cast<double*>(p.v_work[0]), reinterpret_cast<double*>(p.v_work[1])};
-  double* part_m = reinterpret_cast<double*>(p.part_m);
-  double* part_s = reinterpret_cast<double*>(p.part_s);
-  float* dmin_u = reinterpret_cast<float*>(p.err_ring + 8);  // [nblk] per-CTA min of (u_new - u_old)
-  float* dmin_v = dmin_u + 512;                                // [nblk] per-CTA min of (v_new - v_old)
 
   Xf<true> xf;
   const float cmax = p.cost_max ? __ldg(p.cost_max) : 1.f;
@@ -573,18 +589,9 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
   const float nr = -1.f / (p.reg * (p.normalize ? cmax : 1.f));
   const float kBig = 3.0e38f;
 
-  const int base = n0 / nblk, rem = n0 % nblk;
-  const int r_begin = b * base + min(b, rem);
-  const int r_end = r_begin + base + (b < rem ? 1 : 0);
+  const SkSlab slab = sk_slab(n0, nblk, b);
+  const int r_begin = slab.begin, r_end = slab.end;
 
-  auto stage_v = [&](const double* v_cur) {
-    for (int j = tid; j < n1p; j += kSkThreads) {
-      const double vj = (j < n1) ? __ldcg(v_cur + j) : 0.0;
-      v_s[j] = vj;
-      vh_s[j] = (float)vj;
-    }
-    __syncthreads();
-  };
   auto global_min = [&](const float* slots) -> float {  // min over the per-CTA slots (after a grid barrier)
     float v = kBig;
     for (int c = tid; c < nblk; c += kSkThreads) v = fminf(v, __ldcg(slots + c));
@@ -612,7 +619,7 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
       }
     }
     dmin = block_min_f(lane == 0 ? dmin : kBig, redf, tid);
-    if (tid == 0) dmin_u[b] = dmin;
+    if (tid == 0) p.dmin_u[b] = dmin;
   };
 
   // column partials over the slab with the u of u_work (use_u) or u = 0; seeded: thr_j = LSE_prev_j + du_min - gap
@@ -637,65 +644,25 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
 #pragma unroll
       for (int k = 0; k < KG; ++k) {
         const int g = tid + kSkThreads * k;
-        const bool gv = g < ng;
         for (int rb = 0; rb < R; rb += 8) {
           float4 c[8];
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            if (gv && rb + q < R) {
-              c[q] = load_cost4<VEC>(p.M + (int64_t)(r0 + rb + q) * p.ldm, g * 4, n1);
-            } else {
-              const float inf = __int_as_float(0x7f800000);
-              c[q] = make_float4(inf, inf, inf, inf);
-            }
-          }
-          float uh[8];
-#pragma unroll
-          for (int q = 0; q < 8; ++q) uh[q] = uh_chunk[rb + q];
+          load_block8<VEC>(c, p, r0 + rb, R - rb, g, g < ng);
           if (!seeded) {  // no previous LSE (the very first column pass): thresholds from the block maxima
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
-              cthr[k][0] = fmaxf(cthr[k][0], fmaf(c[q].x, nr, uh[q]) - kScreenGap);
-              cthr[k][1] = fmaxf(cthr[k][1], fmaf(c[q].y, nr, uh[q]) - kScreenGap);
-              cthr[k][2] = fmaxf(cthr[k][2], fmaf(c[q].z, nr, uh[q]) - kScreenGap);
-              cthr[k][3] = fmaxf(cthr[k][3], fmaf(c[q].w, nr, uh[q]) - kScreenGap);
+              const float uh = uh_chunk[rb + q];
+              cthr[k][0] = fmaxf(cthr[k][0], fmaf(c[q].x, nr, uh) - kScreenGap);
+              cthr[k][1] = fmaxf(cthr[k][1], fmaf(c[q].y, nr, uh) - kScreenGap);
+              cthr[k][2] = fmaxf(cthr[k][2], fmaf(c[q].z, nr, uh) - kScreenGap);
+              cthr[k][3] = fmaxf(cthr[k][3], fmaf(c[q].w, nr, uh) - kScreenGap);
             }
           }
-          unsigned hm = 0;  // bit q: row q of the block holds a candidate in one of the four columns
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const bool le = (fmaf(c[q].x, nr, uh[q]) <= cthr[k][0]) & (fmaf(c[q].y, nr, uh[q]) <= cthr[k][1]) &
-                            (fmaf(c[q].z, nr, uh[q]) <= cthr[k][2]) & (fmaf(c[q].w, nr, uh[q]) <= cthr[k][3]);
-            hm |= (le ? 0u : 1u) << q;
-          }
-          while (__any_sync(0xffffffffu, hm != 0u)) {
-            if (hm != 0u) {
-              const int e = __ffs((int)hm) - 1;
-              hm &= hm - 1u;
-              const float4 c01 = (e & 1) ? ((e & 2) ? c[3] : c[1]) : ((e & 2) ? c[2] : c[0]);
-              const float4 c45 = (e & 1) ? ((e & 2) ? c[7] : c[5]) : ((e & 2) ? c[6] : c[4]);
-              const float4 ce = (e & 4) ? c45 : c01;
-              const float ue = uh_chunk[rb + e];
-              const double ud = u_chunk[rb + e];
-              if (!(fmaf(ce.x, nr, ue) <= cthr[k][0])) lse_take(xf(ce.x, ud), cm[k][0], cs[k][0]);
-              if (!(fmaf(ce.y, nr, ue) <= cthr[k][1])) lse_take(xf(ce.y, ud), cm[k][1], cs[k][1]);
-              if (!(fmaf(ce.z, nr, ue) <= cthr[k][2])) lse_take(xf(ce.z, ud), cm[k][2], cs[k][2]);
-              if (!(fmaf(ce.w, nr, ue) <= cthr[k][3])) lse_take(xf(ce.w, ud), cm[k][3], cs[k][3]);
-            }
-          }
+          col_block_seeded(c, u_chunk + rb, uh_chunk + rb, cthr[k], cm[k], cs[k], xf, nr);
         }
       }
       __syncthreads();  // u_chunk is restaged for the next chunk
     }
-#pragma unroll
-    for (int k = 0; k < KG; ++k) {
-      const int g = tid + kSkThreads * k;
-      if (g >= ng) continue;
-      double* pm = part_m + (int64_t)b * n1p + g * 4;
-      double* ps = part_s + (int64_t)b * n1p + g * 4;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) { pm[c] = cm[k][c]; ps[c] = cs[k][c]; }
-    }
+    store_partials<KG>(p, cm, cs, 0);
   };
 
 
@@ -720,7 +687,7 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
     const int ngh = ((ng + 1) / 2 + 31) / 32 * 32;  // float4 groups of the first half-row
     const int rr = warp & 7, half = warp >> 3;
     float dmin = kBig;
-    unsigned long long* ctl = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(p.err_ring) + 4608) + (b == 0 ? 0 : 16);
+    unsigned long long* ctl = p.tl + (b == 0 ? 0 : 16);
     const bool ctl_on = p.timeline == 2 && (b == 0 || b == nblk - 1) && (tid == 0 || tid == 511);
 #define SK_TLC(slot) do { if (ctl_on && r0 == r_begin + 8) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); ctl[(slot) + (tid == 0 ? 0 : 5)] = t_; } } while (0)
     for (int r0 = r_begin; r0 < r_end; r0 += 8) {
@@ -758,155 +725,53 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
 #pragma unroll
       for (int k = 0; k < KG; ++k) {
         const int g = tid + kSkThreads * k;
-        const bool gv = g < ng;
         float4 c[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          if (gv && q < R) {
-            c[q] = VEC ? __ldg(reinterpret_cast<const float4*>(p.M + (int64_t)(r0 + q) * p.ldm + g * 4))
-                       : load_cost4<VEC>(p.M + (int64_t)(r0 + q) * p.ldm, g * 4, n1);
-          } else {
-            const float inf = __int_as_float(0x7f800000);
-            c[q] = make_float4(inf, inf, inf, inf);
-          }
-        }
-        float uh[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) uh[q] = uh_chunk[q];
-        unsigned hm = 0;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const bool le = (fmaf(c[q].x, nr, uh[q]) <= cthr[k][0]) & (fmaf(c[q].y, nr, uh[q]) <= cthr[k][1]) &
-                          (fmaf(c[q].z, nr, uh[q]) <= cthr[k][2]) & (fmaf(c[q].w, nr, uh[q]) <= cthr[k][3]);
-          hm |= (le ? 0u : 1u) << q;
-        }
-        while (__any_sync(0xffffffffu, hm != 0u)) {
-          if (hm != 0u) {
-            const int e = __ffs((int)hm) - 1;
-            hm &= hm - 1u;
-            const float4 c01 = (e & 1) ? ((e & 2) ? c[3] : c[1]) : ((e & 2) ? c[2] : c[0]);
-            const float4 c45 = (e & 1) ? ((e & 2) ? c[7] : c[5]) : ((e & 2) ? c[6] : c[4]);
-            const float4 ce = (e & 4) ? c45 : c01;
-            const float ue = uh_chunk[e];
-            const double ud = u_chunk[e];
-            if (!(fmaf(ce.x, nr, ue) <= cthr[k][0])) lse_take(xf(ce.x, ud), cm[k][0], cs[k][0]);
-            if (!(fmaf(ce.y, nr, ue) <= cthr[k][1])) lse_take(xf(ce.y, ud), cm[k][1], cs[k][1]);
-            if (!(fmaf(ce.z, nr, ue) <= cthr[k][2])) lse_take(xf(ce.z, ud), cm[k][2], cs[k][2]);
-            if (!(fmaf(ce.w, nr, ue) <= cthr[k][3])) lse_take(xf(ce.w, ud), cm[k][3], cs[k][3]);
-          }
-        }
+        load_block8<VEC, true>(c, p, r0, R, g, g < ng);
+        col_block_seeded(c, u_chunk, uh_chunk, cthr[k], cm[k], cs[k], xf, nr);
       }
       SK_TLC(4);
       // (no third barrier: u_chunk / half_* are rewritten only behind the next chunk's first barrier)
     }
-#pragma unroll
-    for (int k = 0; k < KG; ++k) {
-      const int g = tid + kSkThreads * k;
-      if (g >= ng) continue;
-      double* pm = part_m + (int64_t)b * n1p + g * 4;
-      double* ps = part_s + (int64_t)b * n1p + g * 4;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) { pm[c] = cm[k][c]; ps[c] = cs[k][c]; }
-    }
+    store_partials<KG>(p, cm, cs, 0);
     dmin = block_min_f(lane == 0 ? dmin : kBig, redf, tid);
-    if (tid == 0) dmin_u[b] = dmin;
+    if (tid == 0) p.dmin_u[b] = dmin;
   };
-
-  // combine the per-CTA column partials of a slice of columns -> v_new, marginal error, min of (v_new - v_cur)
-  auto combine = [&](const double* v_cur, double* v_new, bool have_cur, double* err_slot) {
-    const int cpc = (n1 + nblk - 1) / nblk;
-    const int c_begin = b * cpc, c_end = min(n1, c_begin + cpc);
-    double err_local = 0.0;
-    float dmin = kBig;
-    const int sub = tid & 7;
-    for (int j0 = c_begin; j0 < c_end; j0 += (kSkThreads >> 3)) {
-      const int j = j0 + (tid >> 3);
-      const bool act = j < c_end;
-      double m = Tr<true>::init(), s = 0.0;
-      if (act) {
-        for (int c0 = sub; c0 < nblk; c0 += 8 * 4) {
-          double mm[4], ss[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int c = c0 + q * 8;
-            if (c < nblk) {
-              mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
-              ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
-            } else { mm[q] = Tr<true>::init(); ss[q] = 0.0; }
-          }
-          double bm = vmax(vmax(mm[0], mm[1]), vmax(mm[2], mm[3]));
-          bm = vmax(bm, m);
-          double acc = s * expd<true>(m, bm);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) acc += ss[q] * expd<true>(mm[q], bm);
-          s = acc; m = bm;
-        }
-      }
-      double gm = m;
-#pragma unroll
-      for (int o = 4; o > 0; o >>= 1) gm = vmax(gm, __shfl_xor_sync(0xffffffffu, gm, o));
-      double gs = s * expd<true>(m, gm);
-#pragma unroll
-      for (int o = 4; o > 0; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);
-      if (act && sub == 0) {
-        const double vn = logb - lse_fin(gm, gs);
-        v_new[j] = vn;
-        if (have_cur) {
-          const double vc = __ldcg(v_cur + j);
-          dmin = fminf(dmin, __double2float_rd(vn - vc));
-          const double e = expm1(vc - vn) / (double)n1;  // column marginal of (u, v_cur) minus 1/n1
-          err_local += e * e;
-        }
-      }
-    }
-    dmin = block_min_f(dmin, redf, tid);
-    if (tid == 0) dmin_v[b] = dmin;
-    if (err_slot != nullptr) {
-      err_local = warp_sum(err_local);
-      if (lane == 0) red[warp] = err_local;
-      __syncthreads();
-      if (warp == 0) {
-        double t = lane < kSkWarps ? red[lane] : 0.0;
-        t = warp_sum(t);
-        if (lane == 0) atomicAdd(err_slot, t);
-      }
-      __syncthreads();
-    }
+  // the combine, and the per-CTA minimum of the v changes for the next row pass
+  auto combine = [&](const double* v_cur, double* v_new, double* err_slot) {
+    const float dmin = block_min_f(combine_cols<true, true>(p, v_cur, v_new, logb, 1.0, err_slot, red), redf, tid);
+    if (tid == 0) p.dmin_v[b] = dmin;
   };
 
   // ---- prologue: v^0 = logb - LSE_i(Mr_ij + 0) ----
-  if (b == 0 && tid < 4) p.err_ring[tid] = 0.0;
+  sk_ring_init(p);
   col_phase(false, false, 0.f);
   grid.sync();
-  combine(nullptr, v_work[0], false, nullptr);
+  combine(nullptr, v_work[0], nullptr);
   grid.sync();
 
-  int cur = 0, iters = 0;
-  bool converged = false;
-  double err = 1.0, prev_check_err = -1.0;
+  SkLoop L;
+  int cur = 0;
   float du_prev = 0.f;  // global minimum of the u changes of the previous iteration
   // CFM_SK_TL=1: %globaltimer marks of iteration 50 for the first and the last CTA (scripts/c4_timeline.py)
-  unsigned long long* tl = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(p.err_ring) + 4608) + (b == 0 ? 0 : 16);
+  unsigned long long* tl = p.tl + (b == 0 ? 0 : 16);
   const bool tl_on = p.timeline && (b == 0 || b == nblk - 1) && tid == 0;
 #define SK_TL(slot) do { if (tl_on && it == 50) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); tl[slot] = t_; } } while (0)
   for (int it = 0; it < p.max_iters; ++it) {
-    const bool last = (it == p.max_iters - 1);
-    const bool check = (it % p.check_every) == 0;
-    const bool do_col = !last || check;
+    const SkStep st = sk_step(p, it);
     SK_TL(0);
-    stage_v(v_work[cur]);
+    stage_v(v_s, vh_s, v_work[cur], n1, n1p);
     SK_TL(1);
-    const float dv_min = it > 0 ? global_min(dmin_v) : 0.f;
+    const float dv_min = it > 0 ? global_min(p.dmin_v) : 0.f;
     SK_TL(2);
-    const bool fused = it > 0 && do_col;
+    const bool fused = it > 0 && st.do_col;
     if (!fused) {
       row_phase(it > 0, dv_min);
       SK_TL(3);
-      iters = it + 1;
-      if (!do_col) break;
+      L.iters = it + 1;
+      if (!st.do_col) break;
       grid.sync();
       SK_TL(4);
-      du_prev = global_min(dmin_u);
+      du_prev = global_min(p.dmin_u);
       col_phase(true, true, du_prev);
       SK_TL(5);
       grid.sync();
@@ -915,57 +780,34 @@ __device__ void sinkhorn_run_seeded(const SkParams& p, unsigned char* smem_raw) 
       const float du_assumed = du_prev - 8.f;
       fused_phase(dv_min, du_assumed);
       SK_TL(5);
-      iters = it + 1;
+      L.iters = it + 1;
       grid.sync();
       SK_TL(6);
-      du_prev = global_min(dmin_u);   // the true minimum: every CTA reads the same slots and takes the same branch
+      du_prev = global_min(p.dmin_u);  // the true minimum: every CTA reads the same slots and takes the same branch
       if (!(du_prev >= du_assumed)) {  // the assumption was too optimistic (or NaN): column pass again, exact bound
         col_phase(true, true, du_prev);
         grid.sync();
       }
     }
     SK_TL(7);
-    if (b == 0 && tid == 0) p.err_ring[(it + 2) & 3] = 0.0;
-    combine(v_work[cur], v_work[cur ^ 1], true, &p.err_ring[it & 3]);
+    combine(v_work[cur], v_work[cur ^ 1], sk_err_slot(p, it));
     SK_TL(8);
     grid.sync();
     SK_TL(9);
-    if (check) {
-      err = sqrt(__ldcg(&p.err_ring[it & 3]));
-      if (err < p.stop_thr) { converged = true; break; }
-      if (p.stall_tol > 0.0 && prev_check_err >= 0.0 &&
-          err > (1.0 - p.stall_tol) * prev_check_err &&
-          err * sqrt((double)n1) < 1e-5) { converged = true; break; }
-      prev_check_err = err;
-    }
-    if (last) break;
+    if (st.check && sk_check_stops(L, p, it)) break;
+    if (st.last) break;
     cur ^= 1;
   }
 #undef SK_TL
-
-  for (int j = b * kSkThreads + tid; j < n1; j += nblk * kSkThreads) p.log_v[j] = __ldcg(v_work[cur] + j);
-  if (b == 0 && tid == 0) {
-    int flags = 0;
-    if (!converged) flags |= CFM_FLAG_NOT_CONVERGED;
-    if (!(err == err)) flags |= CFM_FLAG_NONFINITE;
-    p.status[0] = flags;
-    p.status[1] = iters;
-    p.status[2] = 2;
-    p.status[3] = 1;  // kernel variant: seeded screening
-    *p.err_out = err;
-  }
+  sk_finish(p, L, v_work[cur], 1.0, 2, 1);  // kernel variant 1: seeded screening
 }
 
 template <bool VEC, int KG>
 __global__ void __launch_bounds__(kSkThreads, 1) sinkhorn_kernel(const SkParams p) {
   extern __shared__ __align__(16) unsigned char sk_smem[];
-  bool precise = p.precise == 1;
-  if (p.precise < 0) {
-    const float cmax = p.cost_max ? __ldg(p.cost_max) : 0.f;
-    const float span = (p.normalize ? 1.f : cmax) / p.reg;
-    precise = !(span <= 64.f);
-  }
-  if (p.run_if == 2 && !precise) return;  // the fast case was taken by sinkhorn_v2_kernel
+  const bool precise = p.precise < 0 ? sk_needs_f64(p.cost_max ? __ldg(p.cost_max) : 0.f, p.normalize, p.reg)
+                                     : p.precise == 1;
+  if (p.fp32_by_v2 && !precise) return;  // the fp32 case was taken by sinkhorn_v2_kernel
   if (precise) {
     // mixed arithmetic on one column panel with v staged in shared memory: the seeded-screening solver
     if (p.mixed && p.screen == 1 && p.v_in_smem && p.n1p <= kSkThreads * 4 * KG) sinkhorn_run_seeded<VEC, KG>(p, sk_smem);
@@ -1001,25 +843,31 @@ __global__ void plan_materialize_kernel(const float* __restrict__ M, int n0, int
 
 size_t sinkhorn_v2_compact_pitch(int n0, int n1);  // sinkhorn_v2.cu
 
+// Workspace.  The control region comes first, at a fixed offset for tools that read it (scripts/c4_timeline.py):
+// 32 timeline marks, the error ring, the per-CTA minima of the u and v changes.
 struct SkLayout {
-  size_t u, v0, v1, pm, ps, ring, mq, mq_bytes, total;
+  size_t tl, ring, dmin_u, dmin_v, u, v0, v1, pm, ps, mq, mq_bytes, total;
 };
 static SkLayout sk_layout(int n0, int n1, int grid) {
   const size_t n1p = (size_t)(n1 + 3) / 4 * 4;
   SkLayout L;
   size_t o = 0;
+  L.tl = o; o += 32 * 8;
+  L.ring = o; o += 256;
+  L.dmin_u = o; o += kSkMaxGrid * 4;
+  L.dmin_v = o; o += kSkMaxGrid * 4;
+  o = align_up(o, 256);
   L.u = o; o += align_up((size_t)n0 * 8, 256);
   L.v0 = o; o += align_up(n1p * 8, 256);
   L.v1 = o; o += align_up(n1p * 8, 256);
   L.pm = o; o += align_up((size_t)grid * n1p * 8, 256);
   L.ps = o; o += align_up((size_t)grid * n1p * 8, 256);
-  L.ring = o; o += 8192;  // err ring (4 doubles) + per-CTA minima of the potential changes (2 x 512 floats)
   L.mq_bytes = (size_t)n0 * sinkhorn_v2_compact_pitch(n0, n1);  // 3-byte cost copy (shapes whose fp32 M streams)
   L.mq = o; o += align_up(L.mq_bytes, 256);
   L.total = o;
   return L;
 }
-static int sk_grid_upper() { return sm_count() * 2; }
+static int sk_grid_upper() { return min(sm_count() * 2, kSkMaxGrid); }
 int sinkhorn_v2_launch(SkParams& p, cudaStream_t s);  // sinkhorn_v2.cu
 
 }  // namespace cfm
@@ -1031,7 +879,7 @@ extern "C" size_t cfm_sinkhorn_workspace_bytes(int n0, int n1) {
 }
 
 template <bool VEC, int KG>
-static int sk_launch(SkParams& p, size_t smem, void* workspace, cudaStream_t s) {
+static int sk_launch(SkParams& p, size_t smem, cudaStream_t s) {
   auto kern = sinkhorn_kernel<VEC, KG>;
   CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 0;
@@ -1040,14 +888,6 @@ static int sk_launch(SkParams& p, size_t smem, void* workspace, cudaStream_t s) 
   int grid = sm_count() * (per_sm > 2 ? 2 : per_sm);
   if (grid > p.n0) grid = p.n0;  // at least one row per CTA
   if (grid > sk_grid_upper()) grid = sk_grid_upper();
-  const SkLayout L = sk_layout(p.n0, p.n1, sk_grid_upper());
-  char* w = reinterpret_cast<char*>(workspace);
-  p.u_work = w + L.u;
-  p.v_work[0] = w + L.v0;
-  p.v_work[1] = w + L.v1;
-  p.part_m = w + L.pm;
-  p.part_s = w + L.ps;
-  p.err_ring = reinterpret_cast<double*>(w + L.ring);
   void* args[] = {(void*)&p};
   CFM_CUDA_OK(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(kSkThreads), args, smem, s));
   note_launches(1);
@@ -1075,39 +915,37 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
   memset(&p, 0, sizeof(p));
   p.M = M; p.n0 = n0; p.n1 = n1; p.ldm = ldm; p.reg = reg; p.cost_max = cost_max;
   p.normalize = normalize; p.max_iters = max_iters; p.stop_thr = stop_thr;
-  p.check_every = check_every; p.precise = precise; p.stall_tol = stall_tol;
+  p.check_every = check_every; p.stall_tol = stall_tol;
   p.log_u = log_u; p.log_v = log_v; p.status = status; p.err_out = err;
   p.n1p = (n1 + 3) / 4 * 4;
   p.vec = ((n1 & 3) == 0) && ((ldm & 3) == 0) && ((reinterpret_cast<uintptr_t>(M) & 15) == 0);
   const SkLayout L = sk_layout(n0, n1, sk_grid_upper());
-  {
-    char* w = reinterpret_cast<char*>(workspace);
-    p.u_work = w + L.u; p.v_work[0] = w + L.v0; p.v_work[1] = w + L.v1;
-    p.part_m = w + L.pm; p.part_s = w + L.ps; p.err_ring = reinterpret_cast<double*>(w + L.ring);
-    p.mq = L.mq_bytes ? reinterpret_cast<unsigned char*>(w + L.mq) : nullptr;
-  }
-  // CFM_SK_TL: timeline marks, read by both kernels (so set before the smem-staged launch)
+  char* w = reinterpret_cast<char*>(workspace);
+  p.tl = reinterpret_cast<unsigned long long*>(w + L.tl);
+  p.err_ring = reinterpret_cast<double*>(w + L.ring);
+  p.dmin_u = reinterpret_cast<float*>(w + L.dmin_u);
+  p.dmin_v = reinterpret_cast<float*>(w + L.dmin_v);
+  p.u_work = w + L.u; p.v_work[0] = w + L.v0; p.v_work[1] = w + L.v1;
+  p.part_m = w + L.pm; p.part_s = w + L.ps;
+  p.mq = L.mq_bytes ? reinterpret_cast<unsigned char*>(w + L.mq) : nullptr;
+  // CFM_SK_TL: timeline marks, read by both kernels
   static int tl = -1;
   if (tl < 0) { const char* e = getenv("CFM_SK_TL"); tl = e ? atoi(e) : 0; }
   p.timeline = tl;
-  // precise: -1 auto, 0 fp32, 1 float64, 2 fp32 on the generic kernel, 3 float64 with fp32 exponentials ("mixed"),
-  // 4 = 3 without the screening of negligible terms
-  p.screen = 1;
-  if (precise == 4) { precise = 3; p.screen = 0; }  // mixed without the fp32 screening (cross-checks)
-  if (precise == 3) { precise = 1; p.precise = 1; p.mixed = 1; }
-  else if (precise < 0) p.mixed = 1;  // auto mode needing float64 potentials: "mixed" (fp32 exponentials of float64 differences)
-  // fast fp32 mode on aligned n1 <= 8192: smem-staged kernel (sinkhorn_v2.cu)
-  if (precise == 2) { precise = 0; p.precise = 0; }  // fast arithmetic, generic kernel (cross-checks)
-  else if (precise != 1) {
-    p.run_if = precise < 0 ? 1 : 0;
+  // precise: -1 auto, 0 fp32, 1 float64, 2 fp32 on the generic kernel, 3 float64 potentials with fp32 exponentials
+  // ("mixed"), 4 = 3 without the screening of negligible terms.  2 and 4 are the cross-check references.
+  const bool auto_mode = precise < 0;
+  const bool f64 = precise == 1 || precise == 3 || precise == 4;
+  p.precise = auto_mode ? -1 : f64 ? 1 : 0;
+  p.mixed = auto_mode || precise == 3 || precise == 4;  // auto mode resolves float64 potentials to "mixed"
+  p.screen = precise != 4;
+  // fp32 on aligned n1 <= 8192: the smem-staged kernel (sinkhorn_v2.cu); in auto mode the generic kernel is launched
+  // behind it and runs only when the device resolves to float64
+  if (!f64 && precise != 2) {
     const int rc = sinkhorn_v2_launch(p, s);
     if (rc < 0) return rc;
-    if (rc == CFM_OK) {
-      if (precise == 0) return CFM_OK;
-      p.run_if = 2;  // auto: the generic kernel below only runs when float64 potentials are needed
-    } else {
-      p.run_if = 0;
-    }
+    if (rc == CFM_OK && !auto_mode) return CFM_OK;
+    p.fp32_by_v2 = rc == CFM_OK;
   }
   const size_t vbytes = (size_t)p.n1p * 12;  // float64 stage + its fp32 copy (screened mixed mode)
   p.v_in_smem = vbytes <= 160 * 1024;
@@ -1115,13 +953,13 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
   const int ng = p.n1p / 4;
   const int kg_need = (ng + kSkThreads - 1) / kSkThreads;
   if (p.vec) {
-    if (kg_need <= 1) return sk_launch<true, 1>(p, smem, workspace, s);
-    if (kg_need <= 2) return sk_launch<true, 2>(p, smem, workspace, s);
-    return sk_launch<true, 4>(p, smem, workspace, s);  // n1 > 8192: several column panels
+    if (kg_need <= 1) return sk_launch<true, 1>(p, smem, s);
+    if (kg_need <= 2) return sk_launch<true, 2>(p, smem, s);
+    return sk_launch<true, 4>(p, smem, s);  // n1 > 8192: several column panels
   }
-  if (kg_need <= 1) return sk_launch<false, 1>(p, smem, workspace, s);
-  if (kg_need <= 2) return sk_launch<false, 2>(p, smem, workspace, s);
-  return sk_launch<false, 4>(p, smem, workspace, s);
+  if (kg_need <= 1) return sk_launch<false, 1>(p, smem, s);
+  if (kg_need <= 2) return sk_launch<false, 2>(p, smem, s);
+  return sk_launch<false, 4>(p, smem, s);
 }
 
 extern "C" int cfm_plan_materialize_f64(const float* M, int n0, int n1, int64_t ldm, float reg,

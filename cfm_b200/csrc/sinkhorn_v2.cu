@@ -135,6 +135,9 @@ __device__ __forceinline__ int multi_row(int lane) {
   return r;
 }
 
+// CTAs the combine step reduces in one round trip (19 partials per lane; no sm_90 part has more SMs)
+constexpr int kV2MaxGrid = 152;
+
 // Ring depth of the 3-byte stream: 2 stages leave room for 2 resident chunks at full width.  3 stages with 1 resident
 // chunk gave a slower C2 step and 4096^2 shard (DESIGN.md §3.2).
 constexpr int kV2QStages = 2;
@@ -148,19 +151,16 @@ constexpr uint32_t v2_head_bytes() {
 // S: depth of the fp32 ring.  kres_max: 3-byte chunks that fit beside the 3-byte ring (resident chunks).
 template <int NT, int KG, int R>
 __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, int S, const int kres_max) {
-  constexpr int kV2Consumers = NT, kV2Threads = NT, kV2Warps = NT / 32;
+  constexpr int kV2Consumers = NT, kV2Warps = NT / 32;
   extern __shared__ __align__(128) unsigned char v2_smem[];
   cg::grid_group grid = cg::this_grid();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nblk = gridDim.x, b = blockIdx.x;
   const int n0 = p.n0, n1 = p.n1, n1p = p.n1p, ng = n1p / 4;
 
-  // device-side mode selection shared with sinkhorn.cu (exactly one of the two kernels works)
-  if (p.run_if != 0) {
-    const float cmax = p.cost_max ? __ldg(p.cost_max) : 0.f;
-    const bool precise = !((p.normalize ? 1.f : cmax) / p.reg <= 64.f);
-    if (precise) return;  // uniform over the whole grid: nobody reaches a grid barrier
-  }
+  // auto mode: the float64 case goes to sinkhorn.cu's kernel, launched behind this one (uniform over the grid:
+  // nobody reaches a grid barrier)
+  if (p.precise < 0 && sk_needs_f64(p.cost_max ? __ldg(p.cost_max) : 0.f, p.normalize, p.reg)) return;
 
   const uint32_t stage_floats = (uint32_t)R * (uint32_t)n1p;
   float2* rowpart = reinterpret_cast<float2*>(v2_smem);  // [2][R][16]
@@ -194,9 +194,8 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   // and pitch are formed where they are used: long-lived values cost registers in the combine step.
   const bool compact = fact && p.mq != nullptr;
 
-  const int base = n0 / nblk, rem = n0 % nblk;
-  const int r_begin = b * base + min(b, rem);
-  const int nrows = base + (b < rem ? 1 : 0);
+  const SkSlab slab = sk_slab(n0, nblk, b);
+  const int r_begin = slab.begin, nrows = slab.end - slab.begin;
   const int nchunks = (nrows + R - 1) / R;
 
   // ---- ring bookkeeping (incremental: no 64-bit div/mod in the hot loop) ----
@@ -256,11 +255,10 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   if (tid == 0)
     for (int q = 0; q < S && may_issue(); ++q) issue_next();  // initial fill (wraps into the next sweep if S > nchunks)
 
-  // CFM_SK_TL (debug aid, scripts/sk_v2_timeline.py): %globaltimer marks of iteration 50 by thread 0, in the err
-  // ring region's spare tail from byte 4608 on (where sinkhorn.cu's kernel keeps its marks): [0, 6) CTA 0 and
-  // [8, 14) the last CTA (sweep start, last chunk consumed, partials stored, barrier-1 exit, combine done, barrier-2
-  // exit), [16] / [17] the earliest / latest last-chunk mark of all CTAs (factored sweep only)
-  unsigned long long* tl = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(p.err_ring) + 4608);
+  // CFM_SK_TL (debug aid, scripts/sk_v2_timeline.py): %globaltimer marks of iteration 50 by thread 0: [0, 6) CTA 0
+  // and [8, 14) the last CTA (sweep start, last chunk consumed, partials stored, barrier-1 exit, combine done,
+  // barrier-2 exit), [16] / [17] the earliest / latest last-chunk mark of all CTAs (factored sweep only)
+  unsigned long long* tl = p.tl;
   bool tl_now = false;
   auto tl_mark = [&](int slot) {
     if (!tl_now) return;
@@ -547,7 +545,9 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   // k in the order of a shuffle butterfly over 8 lanes, the order used when 8 lanes of a warp shared a column.
   static_assert(NT == 512, "the combine maps 512 threads onto 64 columns x 8 CTA residues");
   __shared__ float2 cpart[8][64];
-  auto combine = [&](const float* v_cur, float* v_new, bool have_cur, double* err_slot) {
+  // v_cur not null: the column-marginal error of (u, v_cur) goes to *err_slot
+  auto combine = [&](const float* v_cur, float* v_new, double* err_slot) {
+    const bool have_cur = v_cur != nullptr;
     double err_local = 0.0;
     const int c_begin = cslice[0], c_end = cslice[1];
     const int sub = tid >> 6;
@@ -556,44 +556,25 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
       const bool act = j < c_end;
       float m = -1.0e30f, s = 0.f;
       if (act) {
-        if (nblk <= 152) {
-          // every lane loads ALL its <= 19 (max, sum) pairs before it reduces: ONE L2 round trip per column instead of
-          // three dependent ones (the combine sits between the two grid barriers: its latency is fixed cost per iteration)
-          float mm[19], ss[19];
+        // every lane loads ALL its <= kV2MaxGrid / 8 (max, sum) pairs before it reduces: ONE L2 round trip per column
+        // instead of three dependent ones (the combine sits between the two grid barriers: its latency is fixed cost
+        // per iteration)
+        float mm[kV2MaxGrid / 8], ss[kV2MaxGrid / 8];
 #pragma unroll
-          for (int q = 0; q < 19; ++q) {
-            const int c = sub + q * 8;
-            if (c < nblk) {
-              mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
-              ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
-            } else { mm[q] = -1.0e30f; ss[q] = 0.f; }
-          }
-          float bm = m;
-#pragma unroll
-          for (int q = 0; q < 19; ++q) bm = fmaxf(bm, mm[q]);
-          float acc = 0.f;
-#pragma unroll
-          for (int q = 0; q < 19; ++q) acc += ss[q] * ex2f(mm[q] - bm);
-          s = acc; m = bm;
-        } else
-        for (int c0 = sub; c0 < nblk; c0 += 64) {  // larger grids: 8 independent (max, sum) pairs in flight per lane
-          float mm[8], ss[8];
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const int c = c0 + q * 8;
-            if (c < nblk) {
-              mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
-              ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
-            } else { mm[q] = -1.0e30f; ss[q] = 0.f; }
-          }
-          float bm = m;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) bm = fmaxf(bm, mm[q]);
-          float acc = s * ex2f(m - bm);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) acc += ss[q] * ex2f(mm[q] - bm);
-          s = acc; m = bm;
+        for (int q = 0; q < kV2MaxGrid / 8; ++q) {
+          const int c = sub + q * 8;
+          if (c < nblk) {
+            mm[q] = __ldcg(part_m + (int64_t)c * n1p + j);
+            ss[q] = __ldcg(part_s + (int64_t)c * n1p + j);
+          } else { mm[q] = -1.0e30f; ss[q] = 0.f; }
         }
+        float bm = m;
+#pragma unroll
+        for (int q = 0; q < kV2MaxGrid / 8; ++q) bm = fmaxf(bm, mm[q]);
+        float acc = 0.f;
+#pragma unroll
+        for (int q = 0; q < kV2MaxGrid / 8; ++q) acc += ss[q] * ex2f(mm[q] - bm);
+        s = acc; m = bm;
       }
       cpart[sub][tid & 63] = make_float2(m, s);
       const int jf = j0 + (tid >> 3);  // the column this thread folds when tid % 8 == 0
@@ -620,26 +601,15 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
       }
       if (j0 + 64 < c_end) __syncthreads();  // cpart is rewritten by the next pass (after the last, a grid barrier follows)
     }
-    if (err_slot != nullptr) {
-      err_local = warp_sum(err_local);
-      if (lane == 0) red[warp] = err_local;
-      __syncthreads();
-      if (warp == 0) {
-        double t = lane < kV2Warps ? red[lane] : 0.0;
-        t = warp_sum(t);
-        if (lane == 0) atomicAdd(err_slot, t);
-      }
-      __syncthreads();
-    }
+    if (have_cur) sk_err_add(err_local, err_slot, red);
   };
 
   // ---- prologue: v^0 from u = 0 ----
-  if (b == 0 && tid < 4) p.err_ring[tid] = 0.0;
+  sk_ring_init(p);
   if (p.timeline && b == 0 && tid == 0) { tl[16] = ~0ull; tl[17] = 0ull; }
 
-  int cur = 0, iters = 0;
-  bool converged = false;
-  double err = 1.0, prev_check_err = -1.0;
+  SkLoop L;
+  int cur = 0;
   sweep(false, true, nullptr);
   if (compact) {
     // the 3-byte rows were written through the generic proxy; the bulk copies read them through the async
@@ -674,33 +644,25 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
     }
   }
   grid.sync();
-  combine(nullptr, v_work[0], false, nullptr);
+  combine(nullptr, v_work[0], nullptr);
   grid.sync();
 
   for (int it = 0; it < p.max_iters; ++it) {
-    const bool last = (it == p.max_iters - 1);
-    const bool check = (it % p.check_every) == 0;
-    const bool do_col = !last || check;
+    const SkStep st = sk_step(p, it);
     tl_now = p.timeline && it == 50 && tid == 0;
     tl_mark(0);
-    sweep(true, do_col, v_work[cur]);
-    iters = it + 1;
-    if (!do_col) break;
+    sweep(true, st.do_col, v_work[cur]);
+    L.iters = it + 1;
+    if (!st.do_col) break;
     grid.sync();
     tl_mark(3);
-    if (b == 0 && tid == 0) p.err_ring[(it + 2) & 3] = 0.0;
-    combine(v_work[cur], v_work[cur ^ 1], check, check ? &p.err_ring[it & 3] : nullptr);
+    double* err_slot = sk_err_slot(p, it);
+    combine(st.check ? v_work[cur] : nullptr, v_work[cur ^ 1], err_slot);
     tl_mark(4);
     grid.sync();
     tl_mark(5);
-    if (check) {
-      err = sqrt(__ldcg(&p.err_ring[it & 3]));
-      if (err < p.stop_thr) { converged = true; break; }
-      if (p.stall_tol > 0.0 && prev_check_err >= 0.0 && err > (1.0 - p.stall_tol) * prev_check_err &&
-          err * sqrt((double)n1) < 1e-5) { converged = true; break; }
-      prev_check_err = err;
-    }
-    if (last) break;
+    if (st.check && sk_check_stops(L, p, it)) break;
+    if (st.last) break;
     cur ^= 1;
   }
 
@@ -713,19 +675,8 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
     if (kres > 0) v2_mbar_wait(res_full, 0);
   }
 
-  for (int j = b * kV2Threads + tid; j < n1; j += nblk * kV2Threads)
-    p.log_v[j] = (double)__ldcg(v_work[cur] + j) * kLn2d;
-  if (b == 0 && tid == 0) {
-    int flags = 0;
-    if (!converged) flags |= CFM_FLAG_NOT_CONVERGED;
-    if (!(err == err)) flags |= CFM_FLAG_NONFINITE;
-    p.status[0] = flags;
-    p.status[1] = iters;
-    p.status[2] = 0;
-    p.status[3] = compact ? 4 : fact ? 3 : 2;  // kernel variant: 4 = factored on the 3-byte stream, 3 = factored,
-                                               // 2 = log-domain
-    *p.err_out = err;
-  }
+  // kernel variant: 4 = factored on the 3-byte stream, 3 = factored, 2 = log-domain
+  sk_finish(p, L, v_work[cur], kLn2d, 0, compact ? 4 : fact ? 3 : 2);
 }
 
 template <int NT, int KG, int R>
@@ -750,6 +701,7 @@ static int v2_launch_t(SkParams& p, cudaStream_t s) {
   if (S > 8) S = 8;
   int grid = sm_count();
   if (grid > p.n0) grid = p.n0;
+  if (grid > kV2MaxGrid) return 1;  // more partials per column than the combine holds in registers
   // the 3-byte stream re-carves the prologue's ring: kV2QStages stages, then as many resident chunks as fit (no
   // more than the longest slab has)
   size_t ring = (size_t)S * stage_bytes;

@@ -10,8 +10,8 @@ for _ in range(3):
     sb.sample_plan(x0, x1)
 torch.cuda.synchronize()
 B = next(iter(sb._bufs.values()))
-ring = B["ws_sk"][-8192:].cpu().numpy()
-marks = np.frombuffer(ring[4608:4608 + 256].tobytes(), dtype=np.uint64).reshape(2, 16)
+# the timeline marks open the Sinkhorn workspace: 16 per CTA, CTA 0 then the last CTA
+marks = np.frombuffer(B["ws_sk"][:256].cpu().numpy().tobytes(), dtype=np.uint64).reshape(2, 16)
 for c, tag in ((0, "CTA 0"), (1, "last CTA")):
     for off, who in ((0, "thread 0"), (5, "thread 511")):
         t0 = int(marks[c, 0 + off])

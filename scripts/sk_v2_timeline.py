@@ -19,7 +19,6 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import cfm_b200  # noqa: E402
-from cfm_b200 import _ffi  # noqa: E402
 
 N, D = 8192, 784
 print("package:", os.path.dirname(cfm_b200.__file__))
@@ -31,10 +30,6 @@ x0, x1 = torch.randn(N, D, generator=g).to(dev), torch.randn(N, D, generator=g).
 s = cfm_b200.OTPlanSampler("sinkhorn", reg=0.05, normalize_cost=True, num_iter_max=100, stop_thr=0.0, warn=False)
 M, cmax, _, _ = s._cost(x0, x1, dev)
 bufs = s._last_bufs
-# workspace layout (sinkhorn.cu sk_layout): ..., err ring region (8192 bytes), 3-byte cost copy (n0 x ldc, 256-aligned)
-total = _ffi.lib().cfm_sinkhorn_workspace_bytes(N, N)
-ldc = (3 * N + 15) // 16 * 16
-ring_off = total - (N * ldc + 255) // 256 * 256 - 8192
 names = ["sweep start", "last chunk", "partials stored", "barrier 1", "combine done", "barrier 2"]
 for _ in range(3):
     s._solve_sinkhorn(M, cmax, N, N, 0.05, True, bufs=bufs)
@@ -44,8 +39,8 @@ for run in range(args.runs):
     cp = s._solve_sinkhorn(M, cmax, N, N, 0.05, True, bufs=bufs)
     torch.cuda.synchronize()
     st = cp.status.cpu().tolist()
-    ring = bufs["ws_sk"][ring_off:ring_off + 8192].cpu().numpy()
-    tl = np.frombuffer(ring[4608:4608 + 18 * 8].tobytes(), dtype=np.uint64).astype(np.int64)
+    # the timeline marks open the Sinkhorn workspace
+    tl = np.frombuffer(bufs["ws_sk"][:18 * 8].cpu().numpy().tobytes(), dtype=np.uint64).astype(np.int64)
     first, last, end_min, end_max = tl[0:6], tl[8:14], tl[16], tl[17]
     t0 = min(first[0], last[0])
     rel = lambda t: (int(t) - t0) / 1e3  # noqa: E731
