@@ -394,7 +394,10 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
             for (int h = 0; h < 2; ++h) {
               const int r = rr + h;
               if (r < R) {
-                const float u2 = loga - (kappa + vref + lg2_abs(Srow[h]));  // lse_r = kappa + vref + log2(S_r)
+                // lse_r = kappa + vref + log2(S_r); a NaN row sum (NaN cost) stays NaN: lg2_abs would read its bits
+                // as 1.5 * 2^128 and give every row the same finite u
+                const float S = Srow[h];
+                const float u2 = loga - (kappa + vref + (S == S ? lg2_abs(S) : S));
                 if (!have_uref) { uref = u2; have_uref = true; }         // first row of the slab fixes uref
                 U[r] = r < rv ? ex2f(u2 - uref) : 0.f;  // padding rows: E = 0 and U = 0 (never 0*inf)
                 if (warp == 0 && lane == 0 && r < rv) {
