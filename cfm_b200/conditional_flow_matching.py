@@ -7,11 +7,12 @@ API surface, class names, method names, attribute names (``sigma``, ``ot_sampler
 elementwise torch ops on the inputs' device, evaluated in the same operation order as the
 reference so results are bit-identical given the same pairs, ``t`` and ``eps``.
 
-For fp32 CUDA batches that do not require grad, the stock classes take a fused path (SURVEY section 8
-f-1, csrc/flow.cu): the pair gather ``x0[i], x1[j]``, ``xt`` and ``ut`` are produced by ONE kernel pass
-whose element arithmetic is unfused round-to-nearest fp32 in the reference's association order, so
-the tensors equal the unfused ones bit for bit (tests/test_gpu_parity.py).  Subclasses that override
-``compute_*`` and inputs that need autograd use the plain torch expressions.
+For contiguous fp32 CUDA batches that do not require grad, the stock classes take a fused path
+(SURVEY section 8 f-1, csrc/flow.cu): the pair gather ``x0[i], x1[j]``, ``xt`` and ``ut`` are produced
+by ONE kernel pass whose element arithmetic is unfused round-to-nearest fp32 in the reference's
+association order, so the tensors equal the unfused ones bit for bit (tests/test_gpu_parity.py,
+tests/test_gpu_flow_gather.py).  Subclasses that override ``compute_*``, inputs that need autograd
+and strided inputs (whose ``randn_like`` noise is laid out differently) use the plain torch expressions.
 """
 import math
 import warnings
@@ -70,9 +71,12 @@ class ConditionalFlowMatcher:
     _FUSED_KIND = _ffi.FLOW_ICFM  # which closed form csrc/flow.cu evaluates for this class
 
     def _fused_ok(self, x0, x1):
+        # Contiguous inputs only: the kernel's eps is drawn contiguous, while the reference's randn_like(x0) keeps
+        # a transposed or channels_last layout and fills it in memory order, i.e. puts other normals on each element.
         stock = _STOCK.get(type(self).__name__)
         return (stock is type(self) and x0.is_cuda and x1.is_cuda and x0.dtype == torch.float32
                 and x1.dtype == torch.float32 and x0.shape == x1.shape and x0.dim() >= 2
+                and x0.is_contiguous() and x1.is_contiguous()
                 and not x0.requires_grad and not x1.requires_grad
                 and isinstance(self.sigma, (int, float)))
 
@@ -101,8 +105,7 @@ class ConditionalFlowMatcher:
             t = torch.rand(n).type_as(x0)
         assert len(t) == n, "t has to have batch size dimension"
         shape = (n,) + tuple(x0.shape[1:])
-        eps = torch.randn(shape, dtype=x0.dtype, device=x0.device)  # == randn_like(x0[i])
-        x0c, x1c = x0.contiguous(), x1.contiguous()
+        eps = torch.randn(shape, dtype=x0.dtype, device=x0.device)  # == randn_like(x0[i]): x0 is contiguous
         ra, rb, rs, rc, sig, kon = self._row_coefficients(t.to(x0.device))
         vec = lambda v: None if v is None else v.to(torch.float32).contiguous()  # noqa: E731
         ra, rb, rs, rc = vec(ra), vec(rb), vec(rs), vec(rc)
@@ -113,7 +116,7 @@ class ConditionalFlowMatcher:
             row *= dsz
         with torch.cuda.device(x0.device):
             _ffi.check(_ffi.lib().cfm_flow_pairs_f32(
-                self._FUSED_KIND, _ffi.ptr(x0c), _ffi.ptr(x1c), _ffi.ptr(i), _ffi.ptr(j), _ffi.ptr(eps),
+                self._FUSED_KIND, _ffi.ptr(x0), _ffi.ptr(x1), _ffi.ptr(i), _ffi.ptr(j), _ffi.ptr(eps),
                 _ffi.ptr(ra), _ffi.ptr(rb), _ffi.ptr(rs), _ffi.ptr(rc), sig, kon, _ffi.ptr(xt), _ffi.ptr(ut),
                 n, row, _ffi.stream_ptr(x0.device)), "cfm_flow_pairs_f32")
         return (t, xt, ut, eps) if return_noise else (t, xt, ut)
