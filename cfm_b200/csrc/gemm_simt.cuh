@@ -34,12 +34,12 @@ __device__ __forceinline__ float4 gemm_load4(const float* __restrict__ P, int64_
 template <class Epi>
 __global__ void __launch_bounds__(kGemmThreads, 2)
 gemm_nt_simt_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict__ B,
-                    int64_t ldb, int M, int N, int K, Epi epi) {
+                    int64_t ldb, int M, int N, int K, int m_base, Epi epi) {
   __shared__ __align__(16) float As[2][kGemmBK][kGemmBM];
   __shared__ __align__(16) float Bs[2][kGemmBK][kGemmBN];
 
   const int tid = threadIdx.x;
-  const int m0 = blockIdx.y * kGemmBM;
+  const int m0 = m_base + blockIdx.y * kGemmBM;
   const int n0 = blockIdx.x * kGemmBN;
   const bool a_vec = ((lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0);
   const bool b_vec = ((ldb & 3) == 0) && ((reinterpret_cast<uintptr_t>(B) & 15) == 0);
@@ -120,9 +120,18 @@ gemm_nt_simt_kernel(const float* __restrict__ A, int64_t lda, const float* __res
 template <class Epi>
 inline cudaError_t launch_gemm_nt_simt(const float* A, int64_t lda, const float* B, int64_t ldb,
                                        int M, int N, int K, Epi epi, cudaStream_t s) {
-  dim3 grid((N + kGemmBN - 1) / kGemmBN, (M + kGemmBM - 1) / kGemmBM);
-  gemm_nt_simt_kernel<Epi><<<grid, kGemmThreads, 0, s>>>(A, lda, B, ldb, M, N, K, epi); ::cfm::note_launches(1);
-  return cudaGetLastError();
+  // gridDim.y holds at most 65535 tile rows: a larger M takes one launch per 65535 tile rows, each starting at row
+  // m_base, so every tile is computed exactly as in a single launch
+  const int mtiles = (int)(((int64_t)M + kGemmBM - 1) / kGemmBM);
+  const unsigned ntiles = (unsigned)(((int64_t)N + kGemmBN - 1) / kGemmBN);
+  for (int mt = 0; mt < mtiles; mt += 65535) {
+    const dim3 grid(ntiles, mtiles - mt < 65535 ? mtiles - mt : 65535);
+    gemm_nt_simt_kernel<Epi><<<grid, kGemmThreads, 0, s>>>(A, lda, B, ldb, M, N, K, mt * kGemmBM, epi);
+    ::cfm::note_launches(1);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 }  // namespace cfm

@@ -824,17 +824,19 @@ __global__ void plan_materialize_kernel(const float* __restrict__ M, int n0, int
                                         const double* __restrict__ lu, const double* __restrict__ lv,
                                         double* __restrict__ plan, double* mass, int32_t* status) {
   const float cmax = (normalize && cost_max) ? __ldg(cost_max) : 1.f;
-  const int i = blockIdx.y;
-  const double ui = lu[i];
   double local = 0.0;
   bool bad = false;
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n1; j += gridDim.x * blockDim.x) {
-    float m = M[(int64_t)i * ldm + j];
-    if (normalize) m = __fdiv_rn(m, cmax);
-    const double v = exp((double)(-__fdiv_rn(m, reg)) + ui + lv[j]);
-    plan[(int64_t)i * n1 + j] = v;
-    local += v;
-    bad |= !isfinite(v);
+  // rows beyond gridDim.y's 65535 are taken in steps of gridDim.y (the launch caps it)
+  for (int i = blockIdx.y; i < n0; i += gridDim.y) {
+    const double ui = lu[i];
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n1; j += gridDim.x * blockDim.x) {
+      float m = M[(int64_t)i * ldm + j];
+      if (normalize) m = __fdiv_rn(m, cmax);
+      const double v = exp((double)(-__fdiv_rn(m, reg)) + ui + lv[j]);
+      plan[(int64_t)i * n1 + j] = v;
+      local += v;
+      bad |= !isfinite(v);
+    }
   }
   local = warp_sum(local);
   if ((threadIdx.x & 31) == 0 && local != 0.0) atomicAdd(mass, local);
@@ -971,7 +973,7 @@ extern "C" int cfm_plan_materialize_f64(const float* M, int n0, int n1, int64_t 
   CFM_REQUIRE(n0 > 0 && n1 > 0 && ldm >= n1, "cfm_plan_materialize_f64: bad shape");
   CFM_REQUIRE(!(normalize && !cost_max), "cfm_plan_materialize_f64: normalize needs cost_max");
   CFM_CUDA_OK(cudaMemsetAsync(mass, 0, sizeof(double), s));
-  dim3 grid((n1 + 1023) / 1024 > 8 ? 8 : (n1 + 1023) / 1024, n0);
+  dim3 grid((n1 + 1023) / 1024 > 8 ? 8 : (n1 + 1023) / 1024, n0 < 65535 ? n0 : 65535);
   plan_materialize_kernel<<<grid, 256, 0, s>>>(M, n0, n1, ldm, reg, cost_max, normalize, log_u, log_v,
                                               plan, mass, status); ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());

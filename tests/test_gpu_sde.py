@@ -7,8 +7,11 @@ instantiations in the built library.
 GPU: parity with supplied increments over widths, dimensions, activations and both kinds of ts; bit identity with the
 ODE kernel's Euler; sigma = 0; seeding; row independence across launch shapes (one test per instantiation); the
 device generator's mapping; the increments' statistics; no launch on refusal."""
+import json
+import os
 import re
 import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -22,6 +25,7 @@ from cfm_b200 import _ffi
 from cfm_b200 import sde as csde
 
 DEV = "cuda:0"
+TESTS = os.path.dirname(os.path.abspath(__file__))
 gpu = pytest.mark.gpu
 
 # sde_small_kernel<U, MAXT> instantiations (U = w / 32, MAXT = threads per CTA); the planner gives at most 16 warps
@@ -311,19 +315,55 @@ def _profiled(fn, tmp_path):
     return out, ran
 
 
-@gpu
-@pytest.mark.parametrize("u,maxt", SDE_KERNELS)
-def test_rows_are_independent_of_the_launch_shape(u, maxt, tmp_path):
-    """Each instantiation runs once (the profiler names it); the first rows of that batch equal a small run with the
-    same seed, which the planner launches with 4 warps per CTA, and the float64 oracle on the device's own noise."""
+def _rows_case(u, maxt):
+    """(sde, float64 sde, y0, ts) of test_rows_are_independent_of_the_launch_shape."""
     w, dim, sms = 32 * u, 3, _sms()
     # 256 threads: 8 warps per CTA, one row group each; 512 threads: 16 warps with three row groups each
     B = 12 * sms + 1 if maxt == 256 else 80 * sms + 3
     sde, f64 = _sde(dim, w, seed=100 + u, act="silu" if u == 2 else "selu")
     y0 = torch.randn(B, dim, generator=torch.Generator().manual_seed(101)).to(DEV)
-    ts = torch.tensor([0.0, 0.1, 0.25])
+    return sde, f64, y0, torch.tensor([0.0, 0.1, 0.25])
+
+
+def _trace_all(tmp_dir):
+    """Run in a child process: one traced sdeint of every SDE_KERNELS case, saved as <u>_<maxt>.pt; prints
+    {"<u>_<maxt>": kernels} as JSON."""
+    import pathlib
+    out = {}
+    for u, maxt in SDE_KERNELS:
+        sde, _, y0, ts = _rows_case(u, maxt)
+        torch.manual_seed(7)
+        big, out[f"{u}_{maxt}"] = _profiled(lambda: cfm_b200.sdeint(sde, y0, ts, method="euler", dt=0.02),
+                                            pathlib.Path(tmp_dir))
+        torch.save(big.cpu(), pathlib.Path(tmp_dir) / f"{u}_{maxt}.pt")
+    print(json.dumps(out))
+
+
+@pytest.fixture(scope="module")
+def traces(tmp_path_factory):
+    """"<u>_<maxt>" -> (kernels, trajectory), traced in a child process: once a process has taken a trace, kernels go
+    missing from its later traces (tests/test_gpu_flow_gather.py), so the pytest process takes none.  The trajectories
+    come back so that each test can check that its own run computed the traced run's bits."""
+    tmp = tmp_path_factory.mktemp("traces")
+    code = "import sys; sys.path[:0] = sys.argv[1:3]; import test_gpu_sde as t; t._trace_all(sys.argv[3])"
+    r = subprocess.run([sys.executable, "-c", code, os.path.dirname(TESTS), TESTS, str(tmp)], capture_output=True,
+                       text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-4000:]
+    ran = json.loads(r.stdout.strip().splitlines()[-1])
+    return {name: ([tuple(k) for k in ks], torch.load(tmp / f"{name}.pt")) for name, ks in ran.items()}
+
+
+@gpu
+@pytest.mark.parametrize("u,maxt", SDE_KERNELS)
+def test_rows_are_independent_of_the_launch_shape(u, maxt, traces):
+    """Each instantiation runs once (the profiler names it); the first rows of that batch equal a small run with the
+    same seed, which the planner launches with 4 warps per CTA, and the float64 oracle on the device's own noise."""
+    sde, f64, y0, ts = _rows_case(u, maxt)
+    B, dim = y0.shape
     torch.manual_seed(7)
-    big, ran = _profiled(lambda: cfm_b200.sdeint(sde, y0, ts, method="euler", dt=0.02), tmp_path)
+    big, n = _launches(lambda: cfm_b200.sdeint(sde, y0, ts, method="euler", dt=0.02))
+    ran, traced = traces[f"{u}_{maxt}"]
+    assert n == 1 and torch.equal(traced, big.cpu())
     assert len(ran) == 1 and ran[0][:2] == (u, maxt), ran
     for k in (1, 7, 333):
         torch.manual_seed(7)

@@ -14,8 +14,10 @@ Batch sizes follow from the device's SM count or from the library's own plan que
 on a part with a different SM count."""
 import itertools
 import json
+import os
 import re
 import subprocess
+import sys
 
 import pytest
 import torch
@@ -27,6 +29,7 @@ import cfm_b200
 from cfm_b200 import _ffi
 
 DEV = "cuda:0"
+TESTS = os.path.dirname(os.path.abspath(__file__))
 gpu = pytest.mark.gpu
 
 # ode_small_kernel<U, MAXT, false> instantiations (U = w / 32, MAXT = threads per CTA).  w = 128 has no 1024-thread
@@ -73,6 +76,45 @@ def _profiled(fn, tmp_path):
             ran.append((int(m.group(1)), int(m.group(2)), m.group(3) == "true", e["args"]["grid"][0],
                         e["args"]["block"][0]))
     return out, ran
+
+
+def _traced_cases():
+    """name -> (case kind in _CASES, its arguments) of every test here that reads the kernel from a trace."""
+    sms = _sms()
+    cases = {f"plain_{u}_{maxt}": ("plain", (u, maxt)) for u, maxt in PLAIN_KERNELS}
+    for which, B, act in (("above_4_warps", 24 * sms + 1, "selu"),
+                          ("half_of_bmax", _cnf_bmax(3, 128) // 2 | 1, "silu")):
+        cases[f"cnf_{which}"] = ("cnf", (128, 3, B, act, 500))
+    return cases
+
+
+def _trace_all(tmp_dir):
+    """Run in a child process: one traced trajectory of every _traced_cases() case, saved as <name>.pt; prints
+    {name: kernels} as JSON."""
+    import pathlib
+    out = {}
+    for name, (kind, args) in _traced_cases().items():
+        _, _, x, _, span, node = _CASES[kind](*args)
+        xd = x.to(DEV)
+        traj, out[name] = _profiled(lambda: node.trajectory(xd, span), pathlib.Path(tmp_dir))
+        torch.save(traj.cpu(), pathlib.Path(tmp_dir) / f"{name}.pt")
+        del node
+    print(json.dumps(out))
+
+
+@pytest.fixture(scope="module")
+def traces(tmp_path_factory):
+    """name -> (kernels, trajectory) of every _traced_cases() case, traced in a child process: once a process has taken
+    a trace, kernels go missing from its later traces (tests/test_gpu_flow_gather.py), and test files that run before
+    this one take traces in the pytest process.  The trajectories come back so that each test can check that its own
+    run computed the traced run's bits."""
+    tmp = tmp_path_factory.mktemp("traces")
+    code = "import sys; sys.path[:0] = sys.argv[1:3]; import test_gpu_small_fields as t; t._trace_all(sys.argv[3])"
+    r = subprocess.run([sys.executable, "-c", code, os.path.dirname(TESTS), TESTS, str(tmp)], capture_output=True,
+                       text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-4000:]
+    ran = json.loads(r.stdout.strip().splitlines()[-1])
+    return {name: ([tuple(k) for k in ks], torch.load(tmp / f"{name}.pt")) for name, ks in ran.items()}
 
 
 def _launches(fn):
@@ -204,21 +246,26 @@ def test_cnf_dopri5_matches_the_float64_oracle_step_for_step(w, dim, span, act):
 
 
 # ---- exact-likelihood variant: the planner's edges -------------------------------------------------------------
-def _check_cnf_euler_batch(w, dim, B, act, seed, tmp_path=None):
-    """Euler over 3 points at batch B: one launch, sampled rows and the last 7 against the float64 oracle, the first
-    333 rows alone bit-identical.  With ``tmp_path``, returns the threads per CTA the profiler saw."""
+def _cnf_case(w, dim, B, act, seed):
+    """(MLP, float64 MLP, state z, generator past z, span, node) of _check_cnf_euler_batch."""
     m, mc = _pair(dim, w, seed=seed, act=act)
     g = torch.Generator().manual_seed(seed)
     z = _state(torch.randn(B, dim, generator=g))
-    span = torch.linspace(1, 0, 3)
-    node = cfm_b200.NeuralODE(cfm_b200.cnf_wrapper(m), solver="euler")
+    return m, mc, z, g, torch.linspace(1, 0, 3), cfm_b200.NeuralODE(cfm_b200.cnf_wrapper(m), solver="euler")
+
+
+def _check_cnf_euler_batch(w, dim, B, act, seed, traced=None):
+    """Euler over 3 points at batch B: one launch, sampled rows and the last 7 against the float64 oracle, the first
+    333 rows alone bit-identical.  With ``traced`` (kernels, trajectory) from the traces fixture, returns the threads
+    per CTA the profiler saw."""
+    m, mc, z, g, span, node = _cnf_case(w, dim, B, act, seed)
     zd = z.to(DEV)
     block = None
-    if tmp_path is None:
-        traj, n = _launches(lambda: node.trajectory(zd, span))
-        assert n == 1
-    else:
-        traj, ran = _profiled(lambda: node.trajectory(zd, span), tmp_path)
+    traj, n = _launches(lambda: node.trajectory(zd, span))
+    assert n == 1
+    if traced is not None:
+        ran, traced_traj = traced
+        assert torch.equal(traced_traj, traj.cpu())
         assert len(ran) == 1 and ran[0][:3] == (w // 32, 256, True), ran
         grid, block = ran[0][3:]
         assert grid <= _sms() and block % 32 == 0 and block <= 256, ran
@@ -250,11 +297,12 @@ def test_cnf_largest_planned_batch_and_the_first_refused_one(w, dim, record_prop
 
 @gpu
 @pytest.mark.parametrize("which", ["above_4_warps", "half_of_bmax"])
-def test_cnf_fewer_warps_fallback(which, tmp_path, record_property):
+def test_cnf_fewer_warps_fallback(which, traces, record_property):
     """w = 128, dim = 3: 8 warps of tangent buffers do not fit next to the weights, so the planner runs fewer warps
     per CTA with more row groups each."""
     B = 24 * _sms() + 1 if which == "above_4_warps" else _cnf_bmax(3, 128) // 2 | 1
-    block = _check_cnf_euler_batch(128, 3, B, "selu" if which == "above_4_warps" else "silu", 500, tmp_path)
+    block = _check_cnf_euler_batch(128, 3, B, "selu" if which == "above_4_warps" else "silu", 500,
+                                   traces[f"cnf_{which}"])
     record_property("threads_per_cta", block)
     assert block < 256
 
@@ -270,17 +318,28 @@ def _plain_warps(B, sms):
     return next(n for n in (4, 8, 16, 32) if groups <= n * sms)
 
 
+def _plain_case(u, maxt):
+    """(MLP, float64 MLP, x, None, span, dopri5 node) of test_plain_instantiation_vs_float64_oracle."""
+    w, dim = 32 * u, {1: 5, 2: 3, 4: 8}[u]
+    m, mc = _pair(dim, w, seed=600 + maxt + u, act="silu" if PLAIN_KERNELS.index((u, maxt)) % 2 else "selu")
+    x = torch.randn(_plain_batch(maxt, _sms()), dim, generator=torch.Generator().manual_seed(700 + u))
+    node = cfm_b200.NeuralODE(cfm_b200.torch_wrapper(m), solver="dopri5", atol=1e-4, rtol=1e-4)
+    return m, mc, x, None, torch.linspace(0, 1, 4), node
+
+
+_CASES = {"cnf": _cnf_case, "plain": _plain_case}
+
+
 @gpu
 @pytest.mark.parametrize("u,maxt", PLAIN_KERNELS)
-def test_plain_instantiation_vs_float64_oracle(u, maxt, tmp_path):
-    w, dim, sms = 32 * u, {1: 5, 2: 3, 4: 8}[u], _sms()
+def test_plain_instantiation_vs_float64_oracle(u, maxt, traces):
+    sms = _sms()
     B = _plain_batch(maxt, sms)
-    m, mc = _pair(dim, w, seed=600 + maxt + u, act="silu" if PLAIN_KERNELS.index((u, maxt)) % 2 else "selu")
-    x = torch.randn(B, dim, generator=torch.Generator().manual_seed(700 + u))
+    m, mc, x, _, span, node = _plain_case(u, maxt)
     xd = x.to(DEV)
-    span = torch.linspace(0, 1, 4)
-    node = cfm_b200.NeuralODE(cfm_b200.torch_wrapper(m), solver="dopri5", atol=1e-4, rtol=1e-4)
-    traj, ran = _profiled(lambda: node.trajectory(xd, span), tmp_path)
+    traj = node.trajectory(xd, span)
+    ran, traced = traces[f"plain_{u}_{maxt}"]
+    assert torch.equal(traced, traj.cpu())
     assert ran == [(u, maxt, False, ran[0][3], 32 * _plain_warps(B, sms))], ran
     f = lambda t, z: vf.wrapped_forward(mc, t, z)  # noqa: E731
     ref, st = vf.dopri5_trajectory(f, x.double(), span.double(), 1e-4, 1e-4)
