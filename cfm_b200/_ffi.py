@@ -76,6 +76,9 @@ SIGNATURES = {
     "cfm_ode_small_cnf_supported": (_i, [_i64, _i, _i]),
     "cfm_ode_small_cnf_trajectory_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _i64, _p, _i, _f, _f, _i, _p, _p, _p, _sz,
                                                           _p]),
+    "cfm_ode_small_cnf_backward_supported": (_i, [_i64, _i, _i]),
+    "cfm_ode_small_cnf_backward_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
+    "cfm_ode_small_cnf_euler_backward_f32": (_i, [_p] * 8 + [_i, _i, _i, _p, _i64, _p, _i, _p, _p, _p, _p, _sz, _p]),
     "cfm_ode_small_grad_supported": (_i, [_i64, _i, _i]),
     "cfm_ode_small_grad_trajectory_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _i64, _p, _i, _f, _f, _i, _p, _p, _p,
                                                            _sz, _p]),

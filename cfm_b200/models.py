@@ -268,8 +268,11 @@ class cnf_wrapper(torch.nn.Module):
     log p(x1) = prior.log_prob(x0) + ll.
 
     ``forward(t, x)`` is plain PyTorch (torch.func per row), so maximum-likelihood training backpropagates through it
-    on any device.  Under ``torch.no_grad()`` on CUDA, ``cfm_b200.NeuralODE`` integrates a wrapped
-    ``MLP(time_varying=True)`` with ``likelihood_estimator="exact"`` in one kernel instead (cfm_b200/ode.py)."""
+    on any device.  On CUDA, ``cfm_b200.NeuralODE`` integrates a wrapped ``MLP(time_varying=True)`` with
+    ``likelihood_estimator="exact"`` in one kernel instead (cfm_b200/ode.py).  Under autograd, with
+    ``solver="euler"``, w in {32, 64}, dim <= 8 and out_dim == dim, that trajectory is differentiable: ``backward()``
+    gives the exact gradient of the computed fp32 Euler trajectory for the MLP's parameters and the initial state in
+    one more kernel (csrc/cnf_train.cu); for dopri5 and other shapes it raises ``NotImplementedError``."""
 
     def __init__(self, model, likelihood_estimator="exact"):
         super().__init__()

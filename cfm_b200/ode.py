@@ -24,10 +24,20 @@ A decreasing ``t_span`` is integrated as torchdyn does: dopri5 runs the field f_
 s = -t_span (for the MLP only a different weight set, ``MLP._time_reversed``), because the step controller
 only steps forwards.  For an action s the same weight set gives -s(-t, x), whose gradient is the reversed field.
 Euler needs no such step: a negative step already gives the same bits.
+
+Everything here runs without autograd, except one case: the ``cnf_wrapper(mlp, "exact")`` trajectory with autograd
+enabled and ``x`` or a parameter of ``mlp`` requiring grad is attached to the graph (the forward is the same launch
+with the same bits).  For ``solver="euler"`` and ``mlp`` in the backward class -- ``MLP(time_varying=True)``, w in
+{32, 64}, dim <= 8, out_dim == dim, SELU or SiLU, a batch the backward plans -- ``backward()`` gives the exact gradient
+of the computed fp32 Euler trajectory (torchdyn's ``sensitivity="autograd"``; it is returned for
+``sensitivity="adjoint"`` too, whose continuous adjoint differs by O(h)) for the eight parameters and ``x``, in one
+launch of csrc/cnf_train.cu.  Outside the class (dopri5, w = 128, larger batches) ``backward()`` raises
+``NotImplementedError`` with the reason.  ``t_span`` requiring grad raises ``ValueError``: there are no time gradients.
 """
 import ctypes as C
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _ffi
 from .models import MLP, GradModel, cnf_wrapper, torch_wrapper
@@ -84,7 +94,12 @@ def _rk_stats(cur, **extra):
 
 
 class NeuralODE(torch.nn.Module):
-    """Subset of torchdyn.core.NeuralODE used by the reference examples."""
+    """Subset of torchdyn.core.NeuralODE used by the reference examples.  ``forward`` returns ``(t_span, traj)``.
+
+    Trajectories are detached, except those of ``cnf_wrapper(mlp, "exact")`` under autograd, which the maximum-likelihood
+    tutorial trains through: with ``solver="euler"`` and ``mlp`` in the backward class (see the module docstring)
+    gradients reach ``mlp``'s parameters and the initial state; otherwise ``backward()`` raises
+    ``NotImplementedError``."""
 
     def __init__(self, vector_field, solver="dopri5", sensitivity="adjoint", atol=1e-4, rtol=1e-4,
                  **unused):
@@ -93,7 +108,7 @@ class NeuralODE(torch.nn.Module):
         if solver not in ("dopri5", "euler"):
             raise NotImplementedError(f"solver {solver!r}: the CUDA driver provides 'dopri5' and 'euler'")
         self.solver, self.atol, self.rtol = solver, float(atol), float(rtol)
-        self.sensitivity = sensitivity  # irrelevant under no_grad sampling; kept for API parity
+        self.sensitivity = sensitivity  # kept for API parity: cnf_wrapper gradients are the discrete (autograd) ones
         self.stats = {}
         self.use_cuda_graph = True  # replay one captured dopri5 step per iteration
         self.max_burst = 32         # steps enqueued between two host reads of the controller state
@@ -109,13 +124,47 @@ class NeuralODE(torch.nn.Module):
         self.lockstep = None
         self._plans = {}
 
-    @torch.no_grad()
     def forward(self, x, t_span):
         traj = self.trajectory(x, t_span)
-        return t_span.to(x.device), traj
+        with torch.no_grad():
+            return t_span.to(x.device), traj
 
-    @torch.no_grad()
     def trajectory(self, x, t_span):
+        """(n_span, *x.shape) states at the ``t_span`` points.  Detached, except for ``cnf_wrapper(mlp, "exact")``
+        under autograd when ``x`` or a parameter of ``mlp`` requires grad: then the trajectory is on the graph.
+        With ``solver="euler"`` and ``mlp`` in the backward class (``cfm_ode_small_cnf_backward_supported``: w in
+        {32, 64}, dim <= 8, out_dim == dim, SELU or SiLU) ``backward()`` computes the exact gradient of the computed
+        fp32 Euler trajectory in one launch, whatever ``sensitivity`` says; outside the class it raises
+        ``NotImplementedError`` with the reason.  The forward is the same launch with the same bits either way."""
+        if isinstance(self.vf, cnf_wrapper) and torch.is_grad_enabled():
+            mlp = _unwrap_cnf(self.vf)
+            params = list(mlp.parameters())
+            if torch.is_tensor(x) and (x.requires_grad or any(p.requires_grad for p in params)):
+                if torch.is_tensor(t_span) and t_span.requires_grad:
+                    raise ValueError("cnf_wrapper: t_span requires grad, but gradients flow to the state and the "
+                                     "model's parameters only; detach it")
+                reason = self._cnf_backward_gap(mlp, x)
+                if reason is None:
+                    return _CnfEulerTrajectory.apply(self, mlp, x, t_span, *params)
+                return _NoBackward.apply(reason, lambda: self._trajectory(x, t_span), x, *params)
+        with torch.no_grad():
+            return self._trajectory(x, t_span)
+
+    def _cnf_backward_gap(self, mlp, x):
+        """Why backward() through this cnf_wrapper trajectory is not implemented, or None when it is."""
+        if self.solver != "euler":
+            return (f"gradients through the adaptive {self.solver} solve are not implemented; use solver='euler'")
+        B = x.shape[0] if x.dim() == 2 else 0
+        if not (mlp.w in (32, 64) and 1 <= mlp.dim <= 8 and mlp.out_dim == mlp.dim
+                and mlp.act in (_ffi.ACT_SELU, _ffi.ACT_SILU)
+                and _ffi.lib().cfm_ode_small_cnf_backward_supported(B, mlp.dim, mlp.w)):
+            return (f"gradients through the exact-likelihood trajectory are not implemented for B={B}, "
+                    f"dim={mlp.dim}, w={mlp.w}, out_dim={mlp.out_dim}; the backward kernel takes w in {{32, 64}}, "
+                    "dim <= 8, out_dim == dim, SELU or SiLU and the batches cfm_ode_small_cnf_backward_supported "
+                    "accepts")
+        return None
+
+    def _trajectory(self, x, t_span):
         cnf = isinstance(self.vf, cnf_wrapper)
         gm = None if cnf else _grad_model(self.vf)
         mlp = _unwrap_cnf(self.vf) if cnf else _unwrap_grad(gm) if gm is not None else _unwrap(self.vf)
@@ -397,6 +446,62 @@ class NeuralODE(torch.nn.Module):
         P["last_steps"] = int(cur.accepted) + int(cur.rejected)
         self.stats = _rk_stats(cur, graph=P["graph"] is not None and not lock, lockstep=lock)
         return traj.clone()
+
+
+class _CnfEulerTrajectory(torch.autograd.Function):
+    """The Euler trajectory of ``cnf_wrapper(mlp, "exact")`` on the graph of ``x`` and the eight parameters of ``mlp``.
+    forward is the one-launch CNF kernel, exactly as without autograd; backward is one call of
+    ``cfm_ode_small_cnf_euler_backward_f32`` (csrc/cnf_train.cu), which reads every state it needs from the saved
+    trajectory and fills a flat gradient buffer in ``parameters()`` order plus the input gradient."""
+
+    @staticmethod
+    def forward(ctx, node, mlp, x, t_span, *params):
+        if not x.is_cuda:
+            raise _ffi.CfmLibraryError("NeuralODE.trajectory needs CUDA inputs (no CPU fallback)")
+        dev = x.device
+        with torch.cuda.device(dev):
+            ts = torch.as_tensor(t_span, dtype=torch.float32).to(dev).contiguous()
+            traj = node._cnf_trajectory_on(mlp, x, ts, dev)
+        ctx.mlp, ctx.ts, ctx.x_dtype = mlp, ts, x.dtype
+        ctx.save_for_backward(traj, *params)  # an in-place update of a parameter before backward() raises
+        return traj
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_traj):
+        traj, *params = ctx.saved_tensors
+        mlp, L = ctx.mlp, _ffi.lib()
+        n_span, B, _ = traj.shape
+        dev = traj.device
+        grads = torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev)
+        gz = torch.empty_like(traj[0]) if ctx.needs_input_grad[2] else None
+        ws = _ffi.workspace(L.cfm_ode_small_cnf_backward_workspace_bytes(B, n_span, mlp.dim, mlp.w), dev)
+        grad_traj = grad_traj.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            _ffi.check(L.cfm_ode_small_cnf_euler_backward_f32(
+                *[_ffi.ptr(p) for p in params], mlp.dim, mlp.w, mlp.act, _ffi.ptr(traj), B, _ffi.ptr(ctx.ts), n_span,
+                _ffi.ptr(grad_traj), _ffi.ptr(gz), _ffi.ptr(grads), _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)),
+                "cfm_ode_small_cnf_euler_backward_f32")
+        out, o = [], 0
+        for p, need in zip(params, ctx.needs_input_grad[4:]):
+            out.append(grads[o:o + p.numel()].view(p.shape) if need else None)
+            o += p.numel()
+        return (None, None, None if gz is None else gz.to(ctx.x_dtype), None, *out)
+
+
+class _NoBackward(torch.autograd.Function):
+    """A trajectory on the graph whose backward() is not implemented: it raises ``NotImplementedError(reason)``
+    instead of torch's generic "does not require grad".  forward is ``run()``, unchanged."""
+
+    @staticmethod
+    def forward(ctx, reason, run, x, *params):
+        ctx.reason = reason
+        return run()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_traj):
+        raise NotImplementedError(ctx.reason)
 
 
 def ctypes_sizeof_state():

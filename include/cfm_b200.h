@@ -319,6 +319,21 @@ int cfm_ode_small_cnf_trajectory_f32(const float* W0, const float* b0, const flo
                                      int64_t batch, const float* t_span, int n_span, float atol,
                                      float rtol, int solver, float* traj, cfm_rk_state* state_out,
                                      void* workspace, size_t workspace_bytes, void* stream);
+/* Gradients through the CNF variant's Euler trajectory (solver = 1, time_varying = 1): given the trajectory traj
+ * [n_span][batch][dim + 1] that cfm_ode_small_cnf_trajectory_f32 wrote for the same weights and t_span, and
+ * grad_traj = dL/dtraj of the same shape, writes dL/dtheta for the eight parameters into grads (flat, in
+ * parameters() order: W0 [w][dim + 1], b0, W1, b1, W2, b2, W3 [dim][w], b3) and, when grad_z is not null, dL/dx0
+ * into grad_z [batch][dim + 1].  The exact gradient of the computed fp32 Euler trajectory (a discrete adjoint over
+ * the stored states), in one cooperative launch with a deterministic fold: the same bits on every call.
+ * supported(): w in {32, 64}, 1 <= dim <= 8 and a batch cfm_ode_small_cnf_supported accepts.  workspace:
+ * cfm_ode_small_cnf_backward_workspace_bytes(). */
+int cfm_ode_small_cnf_backward_supported(int64_t batch, int dim, int w);
+size_t cfm_ode_small_cnf_backward_workspace_bytes(int64_t batch, int n_span, int dim, int w);
+int cfm_ode_small_cnf_euler_backward_f32(const float* W0, const float* b0, const float* W1, const float* b1,
+                                         const float* W2, const float* b2, const float* W3, const float* b3,
+                                         int dim, int w, int act, const float* traj, int64_t batch,
+                                         const float* t_span, int n_span, const float* grad_traj, float* grad_z,
+                                         float* grads, void* workspace, size_t workspace_bytes, void* stream);
 /* Gradient-field variant (action matching: torch_wrapper(GradModel(action)) of the 2-D tutorial): the field is
  * f(t, x) = grad_x s(t, x) of a scalar action s = MLP(dim, out_dim = 1, w, time_varying), evaluated per row by one
  * forward and one reverse pass through the same MLP.  W3 is [1][w] and b3 [1] (b3 does not enter the gradient);
