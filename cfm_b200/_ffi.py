@@ -89,6 +89,9 @@ SIGNATURES = {
     "cfm_mlp_small_train_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
     "cfm_mlp_small_mse_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),
     "cfm_mlp_small_action_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),
+    "cfm_mlp_tc_train_supported": (_i, [_i64, _i, _i, _i]),
+    "cfm_mlp_tc_train_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
+    "cfm_mlp_tc_mse_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),
 }
 
 _lock = threading.Lock()

@@ -45,6 +45,17 @@ __device__ __forceinline__ void split_h3(float v, __half& hi, __half& lo) {
   hi = __float2half_rn(v);
   lo = __float2half_rn((v - __half2float(hi)) * kH3Scale);
 }
+// power-of-two range scale of a producer whose max |value| is am: puts am * scale in [2^13, 2^14) (exact; fp16 tops out
+// at 65504); zero or non-finite am keeps scale 1
+__device__ __forceinline__ float h3_pow2_scale(float am) {
+  float sc = 1.f;
+  if (am > 0.f && am < 3.0e38f) {
+    int e = ilogbf(am);
+    e = max(-100, min(100, 13 - e));
+    sc = scalbnf(1.f, e);
+  }
+  return sc;
+}
 // saturating variant for unscaled producers (activations): |v| > 65504 clamps instead of becoming inf
 // (cvt.rn.satfinite: one instruction per conversion)
 __device__ __forceinline__ __half f2h_satfinite(float v) {

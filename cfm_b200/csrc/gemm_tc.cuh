@@ -16,10 +16,13 @@
 //                    -- store32 is called by the whole warp, which writes the chunk coalesced via tc_store_chunk32.
 //                    Meanwhile the producer already streams the next tile's stages.
 // Tiles are walked M-fastest so the B panel stays hot in L2.
-// Users, through gemm_h3.cuh: the fp16x3 cost matrix and the per-layer MLP.  The PTX wrappers below are shared with
+// Users, through gemm_h3.cuh: the fp16x3 cost matrix, the per-layer MLP and the tensor-core training step
+// (train_tc.cu, the only user of split-K; see gemm_wg_body).  The PTX wrappers below are shared with
 // mlp_h3.cu's fused kernel.
 #pragma once
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -142,11 +145,14 @@ __device__ __forceinline__ void tc_store_chunk32(float* tile, const float (&v)[3
   __syncwarp();
 }
 
-template <class Scheme, class Epi>
-__global__ void __launch_bounds__(kWgThreads, 1)
-gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
-               const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
-               const TcShape p, Epi epi) {
+// Split-K (kSplitK, a compile-time property of the epilogue): the work items are (tile, K-slice) pairs, item i =
+// tile i % tiles, slice i / tiles, and slice s covers K-chunks [s * epi.k_chunks, (s + 1) * epi.k_chunks) of the
+// epi.k_slices * epi.k_chunks >= nk chunks.  Before the epilogue of an item the consumers call epi.begin_slice(s); the
+// epilogue writes a partial result per slice, which a later kernel folds.  Without split-K every item is a whole tile.
+template <class Scheme, class Epi, bool kSplitK>
+__device__ __forceinline__ void gemm_wg_body(const CUtensorMap& map_ah, const CUtensorMap& map_al,
+                                             const CUtensorMap& map_bh, const CUtensorMap& map_bl, const TcShape& p,
+                                             Epi& epi) {
   constexpr int kStages = kWgStages, kStageBytes = kWgStageBytes, kK = Scheme::kKChunk;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* stage_base = smem;
@@ -157,6 +163,17 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.tiles_m * p.tiles_n;
   const int nk = (p.d + kK - 1) / kK;
+  int num_items = num_tiles;
+  if constexpr (kSplitK) num_items = num_tiles * epi.k_slices;
+  // item t -> its tile and the K-chunk range [kc0, kc1)
+  auto item = [&](int t, int& tile, int& kc0, int& kc1) {
+    tile = t; kc0 = 0; kc1 = nk;
+    if constexpr (kSplitK) {
+      tile = t % num_tiles;
+      kc0 = (t / num_tiles) * epi.k_chunks;
+      kc1 = min(nk, kc0 + epi.k_chunks);
+    }
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
@@ -170,9 +187,11 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int tm = t % p.tiles_m, tn = t / p.tiles_m;
-        for (int kc = 0; kc < nk; ++kc) {
+      for (int t = blockIdx.x; t < num_items; t += gridDim.x) {
+        int tile, kc0, kc1;
+        item(t, tile, kc0, kc1);
+        const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
+        for (int kc = kc0; kc < kc1; ++kc) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sb = stage_base + stage * kStageBytes;
           mbar_expect_tx(&full[stage], kStageBytes);
@@ -193,10 +212,12 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
     int stage = 0;
     uint32_t phase = 0;
     float acc0[64], acc1[64];
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int tm = t % p.tiles_m, tn = t / p.tiles_m;
+    for (int t = blockIdx.x; t < num_items; t += gridDim.x) {
+      int tile, kc0, kc1;
+      item(t, tile, kc0, kc1);
+      const int tm = tile % p.tiles_m, tn = tile / p.tiles_m;
       int prev = -1;
-      for (int kc = 0; kc < nk; ++kc) {
+      for (int kc = kc0; kc < kc1; ++kc) {
         mbar_wait(&full[stage], phase);
         const uint32_t sa = smem_u32(stage_base + stage * kStageBytes);
         const uint64_t ah = wg_desc_sw128(sa + wg * 8192), al = wg_desc_sw128(sa + kTileBytes + wg * 8192);
@@ -205,7 +226,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
 #pragma unroll
         for (int k = 0; k < kK / Scheme::kKStep; ++k) {
           const uint64_t koff = (uint64_t)((k * Scheme::kKStep * Scheme::kElem) >> 4);  // 32 bytes per k-step
-          Scheme::mma(acc0, acc1, ah + koff, al + koff, bh + koff, bl + koff, (kc | k) ? 1u : 0u);
+          Scheme::mma(acc0, acc1, ah + koff, al + koff, bh + koff, bl + koff, ((kc - kc0) | k) ? 1u : 0u);
         }
         wg_commit();
         wg_wait<1>();  // the group of the previous chunk has retired: its stage goes back to the producer
@@ -215,6 +236,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
       }
       wg_wait<0>();
       if (prev >= 0) mbar_arrive(&empty[prev]);
+      if constexpr (kSplitK) epi.begin_slice(t / num_tiles);
 
       // ---- epilogue: two 64-column halves through the warpgroup's staging tile ----
       const int fr = 16 * wq + (lane >> 2);  // fragment row (and fr + 8) inside the warpgroup's 64 rows
@@ -255,6 +277,27 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant
   }
 }
 
+template <class Scheme, class Epi>
+__global__ void __launch_bounds__(kWgThreads, 1)
+gemm_wg_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
+               const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
+               const TcShape p, Epi epi) {
+  gemm_wg_body<Scheme, Epi, false>(map_ah, map_al, map_bh, map_bl, p, epi);
+}
+
+// The entry of the epilogues that declare `static constexpr bool kSplitK` (the training GEMMs of train_tc.cu), with or
+// without split-K; the cost-matrix and per-layer MLP epilogues declare nothing and keep gemm_wg_kernel.
+template <class Scheme, class Epi>
+__global__ void __launch_bounds__(kWgThreads, 1)
+gemm_wg_splitk_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
+                      const __grid_constant__ CUtensorMap map_bh, const __grid_constant__ CUtensorMap map_bl,
+                      const TcShape p, Epi epi) {
+  gemm_wg_body<Scheme, Epi, Epi::kSplitK>(map_ah, map_al, map_bh, map_bl, p, epi);
+}
+
+template <class Epi, class = void> struct wg_declares_split_k : std::false_type {};
+template <class Epi> struct wg_declares_split_k<Epi, std::void_t<decltype(Epi::kSplitK)>> : std::true_type {};
+
 // ---- host side -------------------------------------------------------------------------------------
 // launch of gemm_wg_kernel on prepared tensor maps (grid = min(tiles, SMs))
 template <class Scheme, class Epi>
@@ -264,13 +307,19 @@ inline int launch_gemm_wg(const CUtensorMap& mah, const CUtensorMap& mal, const 
   p.n0 = n0; p.n1 = n1; p.d = d;
   p.tiles_m = (n0 + kTM - 1) / kTM;
   p.tiles_n = (n1 + kTN - 1) / kTN;
-  auto kern = gemm_wg_kernel<Scheme, Epi>;
+  int grid = p.tiles_m * p.tiles_n;
+  auto kern = [] {
+    if constexpr (wg_declares_split_k<Epi>::value) return gemm_wg_splitk_kernel<Scheme, Epi>;
+    else return gemm_wg_kernel<Scheme, Epi>;
+  }();
+  if constexpr (wg_declares_split_k<Epi>::value) {
+    if constexpr (Epi::kSplitK) grid *= epi.k_slices;
+  }
   static bool attr_set = false;  // per (Scheme, Epi) instantiation
   if (!attr_set) {
     CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgSmemBytes));
     attr_set = true;
   }
-  int grid = p.tiles_m * p.tiles_n;
   if (grid > sm_count()) grid = sm_count();
   kern<<<grid, kWgThreads, kWgSmemBytes, s>>>(mah, mal, mbh, mbl, p, epi);
   ::cfm::note_launches(1);

@@ -103,12 +103,7 @@ __global__ void prep_rows_h3_kernel(const float* __restrict__ X, int rows, int d
   am = warp_max(am);
   if (uniform_absmax != nullptr) am = __ldg(uniform_absmax);
   // scale = 2^(13 - floor(log2(am))); non-finite or zero rows keep scale 1 (their products are what they are)
-  float sc = 1.f;
-  if (am > 0.f && am < 3.0e38f) {
-    int e = ilogbf(am);
-    e = max(-100, min(100, 13 - e));
-    sc = scalbnf(1.f, e);
-  }
+  const float sc = h3_pow2_scale(am);
   if (lane == 0) {
     if (sqnorm) sqnorm[warp] = s;
     inv_scale[warp] = 1.f / sc;  // exact

@@ -10,15 +10,20 @@ Flow_matching_tutorial.ipynb and SF2M_tutorial.ipynb likewise), as
     loss = cfm_b200.flow_matching_loss(model, xt, t, ut)
     loss.backward()
 
-ONE kernel (csrc/train_small.cu) computes the loss and the gradients of all eight parameters; ``loss`` is attached to
-the autograd graph of the parameters, so ``backward()``, gradient accumulation, clipping, any ``torch.optim``
-optimizer and DDP hooks work as with the eager lines.  The SF2M score loss
-``torch.mean((lambda_t[:, None] * score_model(...) + eps) ** 2)`` is
-``flow_matching_loss(score_model, xt, t, -eps, row_scale=lambda_t)``.
+One library call computes the loss and the gradients of all eight parameters; ``loss`` is attached to the autograd
+graph of the parameters, so ``backward()``, gradient accumulation, clipping, any ``torch.optim`` optimizer and DDP
+hooks work as with the eager lines.  The SF2M score loss ``torch.mean((lambda_t[:, None] * score_model(...) + eps) **
+2)`` is ``flow_matching_loss(score_model, xt, t, -eps, row_scale=lambda_t)``.
 
-Only the tutorial class of model is accelerated: ``cfm_b200.MLP(time_varying=True)`` with ``w`` in {32, 64},
-``dim <= 8`` and ``out_dim <= 8``, fp32 on a CUDA device.  Anything else raises -- there is no eager fallback
-(``MLP.forward`` under autograd is still plain PyTorch for whoever wants it).  Gradients flow to the parameters only.
+Two classes of ``cfm_b200.MLP(time_varying=True)`` (SELU or SiLU, fp32 on a CUDA device) are accelerated:
+
+* small: ``w`` in {32, 64}, ``dim <= 8``, ``out_dim <= 8`` -- ONE kernel (csrc/train_small.cu);
+* tensor-core: the shapes the tensor-core forward samples, ``dim >= 32`` and ``w >= 32`` multiples of 8, ``out_dim`` a
+  multiple of 4, e.g. the MNIST model ``MLP(784, w=256, time_varying=True)`` -- fp16x3 wgmma GEMMs with split-K weight
+  gradients, a fixed 19 launches (csrc/train_tc.cu).
+
+Anything else raises -- there is no eager fallback (``MLP.forward`` under autograd is still plain PyTorch for whoever
+wants it).  Gradients flow to the parameters only.
 
 ``action_matching_loss(action, xt, t, x0, x1)`` does the same for the action-matching cell of the same notebook, whose
 loss needs a double backward: one kernel (csrc/action_train.cu) computes the loss, the input gradient of the action it
@@ -31,19 +36,21 @@ from . import _ffi
 from .models import MLP
 
 
-def _launch(model, params, xt, t, ut, row_scale, with_grad):
-    """One library call: (loss 0-d, flat gradient buffer in parameters() order or None)."""
+def _launch(model, params, xt, t, ut, row_scale, with_grad, kind="small"):
+    """One library call of the class ``kind`` ("small" or "tc"): (loss 0-d, flat gradient buffer in parameters() order
+    or None)."""
     L = _ffi.lib()
+    name = f"cfm_mlp_{kind}_mse_grad_f32"
     dev = xt.device
     B = xt.shape[0]
     loss = torch.empty((), dtype=torch.float32, device=dev)
     grads = torch.empty(sum(p.numel() for p in params), dtype=torch.float32, device=dev) if with_grad else None
-    ws = _ffi.workspace(L.cfm_mlp_small_train_workspace_bytes(B, model.dim, model.w, model.out_dim), dev)
+    ws = _ffi.workspace(getattr(L, f"cfm_mlp_{kind}_train_workspace_bytes")(B, model.dim, model.w, model.out_dim), dev)
     with torch.cuda.device(dev):  # kernels launch on the current device: make it the tensors' one
-        _ffi.check(L.cfm_mlp_small_mse_grad_f32(
+        _ffi.check(getattr(L, name)(
             *[_ffi.ptr(p) for p in params], model.dim, model.w, model.out_dim, model.act, _ffi.ptr(xt), _ffi.ptr(t),
             _ffi.ptr(ut), _ffi.ptr(row_scale), B, 1 if with_grad else 0, _ffi.ptr(loss), _ffi.ptr(grads),
-            _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)), "cfm_mlp_small_mse_grad_f32")
+            _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)), name)
     return loss, grads
 
 
@@ -95,6 +102,21 @@ def _check_model(model, fn="flow_matching_loss", action=False):
             f"{out}, time_varying=True, SELU or SiLU")
 
 
+def _flow_matching_class(model):
+    """"small" or "tc": which kernel trains ``model``; raises NotImplementedError naming both classes otherwise."""
+    if (isinstance(model, MLP) and model.time_varying and model.act in (_ffi.ACT_SELU, _ffi.ACT_SILU)):
+        if model.w in (32, 64) and 1 <= model.dim <= 8 and 1 <= model.out_dim <= 8:
+            return "small"
+        if _ffi.lib().cfm_mlp_tc_train_supported(1, model.dim, model.w, model.out_dim):
+            return "tc"
+    what = (f"MLP(dim={model.dim}, out_dim={model.out_dim}, w={model.w}, time_varying={model.time_varying}, "
+            f"act={model.act})" if isinstance(model, MLP) else type(model).__name__)
+    raise NotImplementedError(
+        f"flow_matching_loss: no training kernel for {what}; it takes cfm_b200.MLP(time_varying=True), SELU or SiLU, "
+        "in one of two classes: small (w in {32, 64}, dim <= 8, out_dim <= 8) or tensor-core (dim >= 32 and w >= 32, "
+        "both multiples of 8, out_dim a multiple of 4)")
+
+
 def _check_tensors(fn, tensors):
     for name, v in tensors:
         if not torch.is_tensor(v):
@@ -122,10 +144,13 @@ def flow_matching_loss(model, xt, t, ut, row_scale=None):
     """``torch.mean((s[:, None] * model(torch.cat([xt, t[:, None]], -1)) - ut) ** 2)`` with ``s = row_scale`` (or 1),
     as a 0-d fp32 CUDA tensor.
 
+    ``model`` is a ``cfm_b200.MLP(time_varying=True)`` with SELU or SiLU of the small class (``w`` in {32, 64},
+    ``dim <= 8``, ``out_dim <= 8``: one kernel) or the tensor-core class (``dim >= 32`` and ``w >= 32`` multiples of 8,
+    ``out_dim`` a multiple of 4: fp16x3 tensor-core GEMMs, 19 launches); anything else raises NotImplementedError.
     ``xt`` (B, dim), ``t`` (B,), ``ut`` (B, out_dim), ``row_scale`` (B,): fp32 on the parameters' CUDA device.  With
-    autograd enabled the result carries the gradients of the model's eight parameters (computed in the same launch as
-    the loss); under ``torch.no_grad()`` the kernel computes the loss only, with the same bits."""
-    _check_model(model)
+    autograd enabled the result carries the gradients of the model's eight parameters (computed in the same call as
+    the loss); under ``torch.no_grad()`` the library computes the loss only, with the same bits."""
+    kind = _flow_matching_class(model)
     tensors = [("xt", xt), ("t", t), ("ut", ut)] + ([("row_scale", row_scale)] if row_scale is not None else [])
     _check_tensors("flow_matching_loss", tensors)
     if xt.dim() != 2 or xt.shape[1] != model.dim or xt.shape[0] < 1:
@@ -141,7 +166,7 @@ def flow_matching_loss(model, xt, t, ut, row_scale=None):
     xt, t, ut = xt.contiguous(), t.contiguous(), ut.contiguous()
     if row_scale is not None:
         row_scale = row_scale.contiguous()
-    return _attach(lambda ps, with_grad: _launch(model, ps, xt, t, ut, row_scale, with_grad), params)
+    return _attach(lambda ps, with_grad: _launch(model, ps, xt, t, ut, row_scale, with_grad, kind), params)
 
 
 def _launch_action(model, params, xt, t, x0, x1, with_grad):

@@ -407,6 +407,23 @@ int cfm_mlp_small_action_grad_f32(const float* W0, const float* b0, const float*
                                   const float* x1, int64_t batch, int with_grad, float* loss, float* grads,
                                   void* workspace, size_t workspace_bytes, void* stream);
 
+/* The same loss, gradients, grads layout, row_scale and with_grad contract as cfm_mlp_small_mse_grad_f32 for WIDE
+ * models, on the tensor cores (fp16x3 wgmma GEMMs, fp32-grade): the class the tensor-core forward samples,
+ * cfm_mlp_tc_supported's shapes (dim >= 32, dim % 8 == 0, w >= 32, w % 8 == 0, out_dim % 4 == 0) with any
+ * 1 <= batch <= 2^30, e.g. MLP(784, w=256, time_varying=True).  A fixed number of launches per call: 19 with
+ * with_grad != 0, 8 without (DESIGN.md section 3.15).  The workspace (cfm_mlp_tc_train_workspace_bytes, 0 outside the
+ * class) must be 16-byte aligned; the weights are split into it anew on every call.  A call repeated on the same
+ * device gives the same bits, and the loss has the same bits with and without gradients.  Argument errors are
+ * reported before any CUDA call. */
+int cfm_mlp_tc_train_supported(int64_t batch, int dim, int w, int out_dim);
+size_t cfm_mlp_tc_train_workspace_bytes(int64_t batch, int dim, int w, int out_dim);
+int cfm_mlp_tc_mse_grad_f32(const float* W0, const float* b0, const float* W1, const float* b1,
+                            const float* W2, const float* b2, const float* W3, const float* b3,
+                            int dim, int w, int out_dim, int act, const float* x, const float* t,
+                            const float* target, const float* row_scale, int64_t batch, int with_grad,
+                            float* loss, float* grads, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif
