@@ -846,16 +846,17 @@ __global__ void plan_materialize_kernel(const float* __restrict__ M, int n0, int
 size_t sinkhorn_v2_compact_pitch(int n0, int n1);  // sinkhorn_v2.cu
 
 // Workspace.  The control region comes first, at a fixed offset for tools that read it (scripts/c4_timeline.py):
-// 32 timeline marks, the error ring, the per-CTA minima of the u and v changes.
+// 32 timeline marks, the error ring (4 doubles) and at byte 288 the count of 22-bit chunks of the cost copy (int32,
+// sinkhorn_v2.cu), the per-CTA minima of the u and v changes.
 struct SkLayout {
-  size_t tl, ring, dmin_u, dmin_v, u, v0, v1, pm, ps, mq, mq_bytes, total;
+  size_t tl, ring, n_narrow, dmin_u, dmin_v, u, v0, v1, pm, ps, mq, mq_bytes, total;
 };
 static SkLayout sk_layout(int n0, int n1, int grid) {
   const size_t n1p = (size_t)(n1 + 3) / 4 * 4;
   SkLayout L;
   size_t o = 0;
   L.tl = o; o += 32 * 8;
-  L.ring = o; o += 256;
+  L.ring = o; L.n_narrow = o + 32; o += 256;
   L.dmin_u = o; o += kSkMaxGrid * 4;
   L.dmin_v = o; o += kSkMaxGrid * 4;
   o = align_up(o, 256);
@@ -925,6 +926,7 @@ extern "C" int cfm_sinkhorn_log_f32(const float* M, int n0, int n1, int64_t ldm,
   char* w = reinterpret_cast<char*>(workspace);
   p.tl = reinterpret_cast<unsigned long long*>(w + L.tl);
   p.err_ring = reinterpret_cast<double*>(w + L.ring);
+  p.n_narrow = reinterpret_cast<int*>(w + L.n_narrow);
   p.dmin_u = reinterpret_cast<float*>(w + L.dmin_u);
   p.dmin_v = reinterpret_cast<float*>(w + L.dmin_v);
   p.u_work = w + L.u; p.v_work[0] = w + L.v0; p.v_work[1] = w + L.v1;

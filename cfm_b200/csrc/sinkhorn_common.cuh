@@ -47,6 +47,8 @@ struct SkParams {
   float l2_resident_frac;  // sinkhorn_v2: share of each slab loaded with L2 evict_last (0: default policy)
   unsigned char* mq;  // sinkhorn_v2: 3-byte fixed-point copy of M (n0 rows of ldc bytes; null: fp32 sweeps only)
   int64_t ldc;        //              its row pitch in bytes, align16(3 * n1)
+  int ldn;            //              bytes of a row whose chunk takes 22-bit entries (0: every chunk keeps 3 bytes)
+  int* n_narrow;      //              control region: chunks of the copy the last solve wrote at 22 bits
   int fp32_by_v2;   // auto mode: sinkhorn_v2_kernel solves the fp32 case, the generic kernel only the float64 one
   int timeline;     // CFM_SK_TL: globaltimer marks of one iteration (debug aid)
   int screen;       // mixed mode: fp32 screening of negligible terms (0 only for precise = 4, the unscreened reference)
@@ -81,9 +83,11 @@ struct SkLoop {
   bool converged = false;
   int iters = 0;
 };
-// prologue: clear the error ring
+// prologue: clear the error ring and the count of 22-bit chunks (every solver, so a solve that writes no copy leaves
+// 0 there; sinkhorn_v2's CTAs add their counts after the grid barrier that follows this)
 __device__ __forceinline__ void sk_ring_init(const SkParams& p) {
   if (blockIdx.x == 0 && threadIdx.x < 4) p.err_ring[threadIdx.x] = 0.0;
+  if (blockIdx.x == 0 && threadIdx.x == 0 && p.n_narrow != nullptr) *p.n_narrow = 0;
 }
 // the error slot of iteration it (between the grid barriers around the combine).  It clears slot it + 2 for later:
 // that slot's last reader, the check of iteration it - 2, is two grid barriers back.

@@ -32,6 +32,11 @@
 //     its fp32 ring the same allocation is re-carved into a kV2QStages-deep ring of 3-byte chunks and as many
 //     chunks resident for the whole solve as fit in the rest: a run of kres slab chunks in the middle of the slab,
 //     filled once, read from shared memory by every later sweep.  Only the other chunks cross the ring (and HBM).
+//   * 22-BIT CHUNKS (KG = 4, where the NT * 44-byte row is shorter than ldc): q = 0 at the largest cost and grows as
+//     the cost falls, so a chunk whose smallest cost encodes below 2^22 never uses the top bit.  The prologue decides
+//     that per chunk (the encode is monotone in M) and writes such a chunk with thread t's 16 entries packed into the
+//     11 words at word 11 t of the row.  Same q, so the same e' and bit-identical results; 8% fewer bytes, and a slab
+//     whose chunks are all narrow re-carves at the narrow pitch (one more resident chunk at C2).
 //   * per-CTA column partials -> [cta][n1] workspace -> grid barrier -> sliced combine -> v_new,
 //     marginal error -> grid barrier (identical to sinkhorn.cu).
 #include <stdlib.h>
@@ -105,6 +110,22 @@ __device__ __forceinline__ uint32_t v2_encode(float m, float c2, float kappa, do
 __device__ __forceinline__ float v2_q_decode(uint32_t w, float qa) {
   return (__uint_as_float(0x4B000000u | (w & 0xFFFFFFu)) - 8388608.f) * qa;
 }
+// the same for a 22-bit entry in the low bits of w (the same float for the same q)
+__device__ __forceinline__ float v2_q22_decode(uint32_t w, float qa) {
+  return (__uint_as_float(0x4B000000u | (w & 0x3FFFFFu)) - 8388608.f) * qa;
+}
+// 22-bit chunks: a thread's 16 entries of a row (4 groups of 4 columns, in column order) fill 11 words, entry i at
+// bit 22 i; the odd stride of 11 words between threads keeps the word loads free of bank conflicts
+constexpr int kV2NarrowWords = 11;
+constexpr uint32_t kV2NarrowRow = 512 * 4 * kV2NarrowWords;  // bytes of a 22-bit row (KG = 4: 512 threads)
+constexpr uint32_t kV2NarrowLimit = 1u << 22;
+// entry i of a thread's 11 words w (i is a constant once the callers' loops are unrolled)
+__device__ __forceinline__ uint32_t v2_q22_field(const uint32_t* w, int i) {
+  const int bit = 22 * i, wd = bit >> 5, sh = bit & 31;
+  return sh + 22 <= 32 ? w[wd] >> sh : __funnelshift_r(w[wd], w[wd + 1], sh);
+}
+// chunks of a slab whose width the per-CTA mask records; a longer slab's later chunks keep 3 bytes
+constexpr int kV2MaskWords = 8;
 
 // Reduce R per-lane values over the warp with a shared shuffle tree: at the stage with offset
 // `off` lanes whose bit `off` is set keep the odd member of each pair, the others the even one, so
@@ -138,8 +159,8 @@ __device__ __forceinline__ int multi_row(int lane) {
 // CTAs the combine step reduces in one round trip (19 partials per lane; no sm_90 part has more SMs)
 constexpr int kV2MaxGrid = 152;
 
-// Ring depth of the 3-byte stream: 2 stages leave room for 2 resident chunks at full width.  3 stages with 1 resident
-// chunk gave a slower C2 step and 4096^2 shard (DESIGN.md §3.2).
+// Ring depth of the 3-byte stream: 2 stages leave room for 2 resident chunks at full width (3 when every chunk of the
+// slab is narrow).  3 stages with 1 resident chunk gave a slower C2 step and 4096^2 shard (DESIGN.md §3.2).
 constexpr int kV2QStages = 2;
 // Head of the dynamic shared memory, the same in every layout: the row partials [2][R][16] and the mbarriers (8 for
 // the fp32 ring, kV2QStages for the 3-byte ring, 1 for the resident chunks).  The stages follow it.
@@ -148,9 +169,10 @@ constexpr uint32_t v2_head_bytes() {
   return (2 * R * (NT / 32) * sizeof(float2) + (8 + kV2QStages + 1) * sizeof(uint64_t) + 127) / 128 * 128;
 }
 
-// S: depth of the fp32 ring.  kres_max: 3-byte chunks that fit beside the 3-byte ring (resident chunks).
+// S: depth of the fp32 ring.  qbytes: dynamic shared memory past the head, which the 3-byte stream re-carves into
+// its ring and resident chunks.
 template <int NT, int KG, int R>
-__global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, int S, const int kres_max) {
+__global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, int S, const int qbytes) {
   constexpr int kV2Consumers = NT, kV2Warps = NT / 32;
   extern __shared__ __align__(128) unsigned char v2_smem[];
   cg::grid_group grid = cg::this_grid();
@@ -170,11 +192,17 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   float* stages = reinterpret_cast<float*>(v2_smem + v2_head_bytes<NT, R>());
   __shared__ double red[kV2Warps];
   __shared__ int cslice[2];  // this CTA's columns in the combine step (in smem: a register there would spill)
+  // 22-bit chunks: bit c of the mask = slab chunk c of the copy is narrow (set by the prologue).  qmode, fixed for
+  // the CTA after the prologue: 0 no narrow chunk (the 3-byte stream as it was), 1 every chunk narrow (stages and
+  // resident chunks at the narrow pitch), 2 mixed (the 3-byte pitch, width looked up per chunk)
+  __shared__ uint32_t nmask[KG == 4 ? kV2MaskWords : 1];
+  __shared__ int qmode;
 
   if (tid == 0) {
     const int cpc = (n1 + nblk - 1) / nblk;
     cslice[0] = b * cpc;
     cslice[1] = min(n1, b * cpc + cpc);
+    for (int w = 0; w < (KG == 4 ? kV2MaskWords : 1); ++w) nmask[w] = 0u;
     for (int s = 0; s < 8 + kV2QStages + 1; ++s) v2_mbar_init(&bars[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -222,14 +250,21 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   // the smem-resident ones; its fp32 prologue is read once and streams entirely.
   // (`l2_end` switches to the 3-byte stream's value when the producer switches format, see below)
   int l2_end = p.l2_resident_frac <= 0.f ? -1 : compact ? 0 : (int)(p.l2_resident_frac * (float)nchunks);
-  // thread 0: issue the bulk copies of the next chunk into its (free) stage
-  auto issue_next = [&]() {
+  // slab chunk c of the copy has 22-bit entries (uniform over the CTA)
+  auto chunk_narrow = [&](int c) {
+    if constexpr (KG == 4) return c < 32 * kV2MaskWords && ((nmask[c >> 5] >> (c & 31)) & 1u) != 0;
+    else return false;
+  };
+  // thread 0: issue the bulk copies of the next chunk into its (free) stage (MODE: the CTA's qmode)
+  auto issue_next = [&](auto MODE) {
+    constexpr int kMode = decltype(MODE)::value;
     const int r0 = r_begin + p_chunk * R;
     const int rv = min(R, r_begin + nrows - r0);
     const bool q = compact && issued >= nchunks;  // the first nchunks chunks are the prologue's
     const uint32_t ldc = (uint32_t)p.ldc;
-    const uint32_t row_bytes = q ? ldc : (uint32_t)n1 * 4u;
-    const uint32_t pitch = q ? ldc : (uint32_t)n1p * 4u;  // a stage is R rows at this pitch
+    const uint32_t qrow = kMode == 1 ? kV2NarrowRow : kMode == 2 && chunk_narrow(p_chunk) ? kV2NarrowRow : ldc;
+    const uint32_t row_bytes = q ? qrow : (uint32_t)n1 * 4u;
+    const uint32_t pitch = q ? (kMode == 1 ? kV2NarrowRow : ldc) : (uint32_t)n1p * 4u;  // a stage: R rows at this pitch
     const uint64_t pol = p_chunk < l2_end ? v2_policy_evict_last() : v2_policy_evict_first();
     v2_mbar_expect_tx(&full[p_st], (uint32_t)rv * row_bytes);
     for (int r = 0; r < rv; ++r) {
@@ -253,7 +288,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   // prologue); the copy is reused from call to call, and an early read would return the previous coupling's rows.
   auto may_issue = [&]() { return issued < nchunks || consumed_total != 0 || !compact; };
   if (tid == 0)
-    for (int q = 0; q < S && may_issue(); ++q) issue_next();  // initial fill (wraps into the next sweep if S > nchunks)
+    for (int q = 0; q < S && may_issue(); ++q) issue_next(std::integral_constant<int, 0>{});  // initial fill (wraps into the next sweep if S > nchunks)
 
   // CFM_SK_TL (debug aid, scripts/sk_v2_timeline.py): %globaltimer marks of iteration 50 by thread 0: [0, 6) CTA 0
   // and [8, 14) the last CTA (sweep start, last chunk consumed, partials stored, barrier-1 exit, combine done,
@@ -298,14 +333,21 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
       // thread about as much as a small shape's sweep has to spare, so only the stream's sweeps form them
       const float qa = fmt != 0 ? (float)((double)(-kappa) / 8388607.0) : 0.f;
       const double qinv = fmt == 1 && qa > 0.f ? 1.0 / (double)qa : 0.0;
+      // the chunk loop, compiled per qmode: mode 0 (every sweep before the stream, and a stream without narrow
+      // chunks) has no width lookup and no 22-bit decode; modes 1 and 2 run only on the stream (fmt 2)
+      auto chunk_loop = [&](auto MODE) {
+      constexpr int kMode = decltype(MODE)::value;
       for (int cc = 0; cc < nchunks; ++cc) {
         const int chunk = (sweep_no & 1) ? nchunks - 1 - cc : cc;
         const int r0 = r_begin + chunk * R;
         const int rv = min(R, r_begin + nrows - r0);
         const bool res = (unsigned)(chunk - rlo) < (unsigned)kres;  // resident: slot S + chunk - rlo, past the ring
+        const bool narrow = kMode == 1 || (kMode == 2 && chunk_narrow(chunk));
+        const uint32_t qp = kMode == 1 ? kV2NarrowRow : ldc;  // row pitch of the copy's chunks in shared memory
         const float* sbase = stages + (uint32_t)c_st * stage_floats + tcol;
-        const unsigned char* qbase =
-            reinterpret_cast<const unsigned char*>(stages) + (uint32_t)(res ? S + chunk - rlo : c_st) * R * ldc + 12 * tid;
+        const unsigned char* qbase = reinterpret_cast<const unsigned char*>(stages) +
+                                     (uint32_t)(res ? S + chunk - rlo : c_st) * R * qp +
+                                     (narrow ? 4 * kV2NarrowWords : 12) * tid;
         float2* rp = rowpart + (cc & 1) * R * kV2Warps;
         if (res) v2_mbar_wait(res_full, 0);
         else v2_mbar_wait(&full[c_st], c_par);
@@ -320,9 +362,16 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
             for (int k = 0; k < KG; ++k) {
               if (!kAll) E[r][k] = make_float4(0.f, 0.f, 0.f, 0.f);
               if (kAll || (gvalid[k] && r < rv)) {
-                if constexpr (kFmt == 2) {
+                if constexpr (kFmt == 3) {
+                  // 22-bit chunk: the group's 4 entries of the thread's 11 words (entry 4k + c at bit 22 (4k + c))
+                  const uint32_t* w = reinterpret_cast<const uint32_t*>(qbase + r * qp);
+                  E[r][k] = make_float4(ex2f(v2_q22_decode(v2_q22_field(w, 4 * k), qa)),
+                                        ex2f(v2_q22_decode(v2_q22_field(w, 4 * k + 1), qa)),
+                                        ex2f(v2_q22_decode(v2_q22_field(w, 4 * k + 2), qa)),
+                                        ex2f(v2_q22_decode(v2_q22_field(w, 4 * k + 3), qa)));
+                } else if constexpr (kFmt == 2) {
                   // 12 bytes = 4 entries; three 4-byte smem loads at a stride of 3 words (no bank conflicts)
-                  const uint32_t* w = reinterpret_cast<const uint32_t*>(qbase + r * ldc + 12 * kV2Consumers * k);
+                  const uint32_t* w = reinterpret_cast<const uint32_t*>(qbase + r * qp + 12 * kV2Consumers * k);
                   const uint32_t w0 = w[0], w1 = w[1], w2 = w[2];
                   E[r][k] = make_float4(ex2f(v2_q_decode(w0, qa)),
                                         ex2f(v2_q_decode(__funnelshift_r(w0, w1, 24), qa)),
@@ -336,7 +385,62 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
               }
             }
         };
-        if (fmt == 1) {
+        bool enc_narrow = false;
+        if constexpr (KG == 4 && kMode == 0) {
+          if (fmt == 1 && p.ldn != 0 && chunk < 32 * kV2MaskWords &&
+              (uint32_t)qbytes >= (uint32_t)S * stage_floats * 4u + (uint32_t)p.ldn) {
+            // the chunk is narrow iff its largest code, the code of its smallest cost (the encode is monotone
+            // non-increasing in M), is below 2^22 and no cost is NaN
+            float mn = __int_as_float(0x7f800000);
+            bool nan = false;
+#pragma unroll 1
+            for (int r = 0; r < rv; ++r)
+#pragma unroll
+              for (int k = 0; k < KG; ++k)
+                if (gvalid[k]) {
+                  const float4 mv = *reinterpret_cast<const float4*>(sbase + r * n1p + kV2Consumers * 4 * k);
+                  mn = fminf(mn, fminf(fminf(mv.x, mv.y), fminf(mv.z, mv.w)));
+                  nan |= (mv.x != mv.x) | (mv.y != mv.y) | (mv.z != mv.z) | (mv.w != mv.w);
+                }
+            enc_narrow = !__syncthreads_or(nan || v2_encode(mn, c2, kappa, qinv) >= kV2NarrowLimit);
+            if (enc_narrow && tid == 0) nmask[chunk >> 5] |= 1u << (chunk & 31);
+          }
+        }
+        if (enc_narrow) {
+          // prologue, 22-bit chunk: thread t's 16 entries of a row into the 11 words at word 11 t (entry i at bit
+          // 22 i; idle groups write 0, so the whole NT * 44-byte row the stream copies is defined).  The row is
+          // packed in shared memory past the fp32 ring and then stored with 16-byte coalesced writes: stored from
+          // registers, each warp store would touch 44 sectors 4 bytes at a time.
+          uint32_t* stg = reinterpret_cast<uint32_t*>(stages + (uint32_t)S * stage_floats);
+#pragma unroll 1
+          for (int r = 0; r < rv; ++r) {
+            uint32_t* dst = stg + kV2NarrowWords * tid;
+            uint32_t acc = 0u;  // the bits of the word being filled
+#pragma unroll
+            for (int k = 0; k < KG; ++k) {
+              uint32_t q[4] = {0u, 0u, 0u, 0u};
+              if (gvalid[k]) {
+                const float4 mv = *reinterpret_cast<const float4*>(sbase + r * n1p + kV2Consumers * 4 * k);
+                q[0] = v2_encode(mv.x, c2, kappa, qinv); q[1] = v2_encode(mv.y, c2, kappa, qinv);
+                q[2] = v2_encode(mv.z, c2, kappa, qinv); q[3] = v2_encode(mv.w, c2, kappa, qinv);
+              }
+#pragma unroll
+              for (int c = 0; c < 4; ++c) {
+                const int bit = 22 * (4 * k + c), sh = bit & 31;
+                acc |= q[c] << sh;
+                if (sh + 22 >= 32) {
+                  dst[bit >> 5] = acc;
+                  acc = sh + 22 > 32 ? q[c] >> (32 - sh) : 0u;
+                }
+              }
+            }
+            v2_consumer_barrier<NT>();
+            const uint4* src4 = reinterpret_cast<const uint4*>(stg);
+            uint4* row4 = reinterpret_cast<uint4*>(p.mq + (int64_t)(r0 + r) * ldc);
+            for (int i = tid; i < p.ldn / 16; i += NT) row4[i] = src4[i];
+            v2_consumer_barrier<NT>();  // the next row reuses the staging words
+          }
+        } else if (kMode == 0 && fmt == 1) {
           // prologue: write this stage's rows into the 3-byte copy (its own pass: E is not live yet)
 #pragma unroll 1
           for (int r = 0; r < rv; ++r)
@@ -355,7 +459,10 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
         using kT = std::true_type;
         using kF = std::false_type;
         const bool all = full_cols && rv == R;  // common case: no predicates in the hot loop
-        if (fmt == 2) { if (all) form_E(std::integral_constant<int, 2>{}, kT{}); else form_E(std::integral_constant<int, 2>{}, kF{}); }
+        if constexpr (kMode != 0) {
+          if (narrow) { if (all) form_E(std::integral_constant<int, 3>{}, kT{}); else form_E(std::integral_constant<int, 3>{}, kF{}); }
+          else if constexpr (kMode == 2) { if (all) form_E(std::integral_constant<int, 2>{}, kT{}); else form_E(std::integral_constant<int, 2>{}, kF{}); }
+        } else if (fmt == 2) { if (all) form_E(std::integral_constant<int, 2>{}, kT{}); else form_E(std::integral_constant<int, 2>{}, kF{}); }
         else { if (all) form_E(std::integral_constant<int, 0>{}, kT{}); else form_E(std::integral_constant<int, 0>{}, kF{}); }
         if (!res && ++c_st == S) { c_st = 0; c_par ^= 1u; }
         if (do_row) {
@@ -376,7 +483,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
         // every warp has now copied its part of the stage into registers: after this barrier the
         // stage is free, so thread 0 refills it with the chunk S positions ahead
         v2_consumer_barrier<NT>();
-        if (tid == 0 && !res && may_issue()) issue_next();
+        if (tid == 0 && !res && may_issue()) issue_next(MODE);
         float U[R];
         if (do_row) {
           // fold the 16 per-warp partials: lanes 0-15 take row r, lanes 16-31 row r+1 (one tree for two rows)
@@ -420,6 +527,15 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
               cs[k][2] = fmaf(E[r][k].z, U[r], cs[k][2]); cs[k][3] = fmaf(E[r][k].w, U[r], cs[k][3]);
             }
         }
+      }
+      };
+      if constexpr (KG == 4) {
+        const int qm = fmt == 2 ? qmode : 0;
+        if (qm == 1) chunk_loop(std::integral_constant<int, 1>{});
+        else if (qm == 2) chunk_loop(std::integral_constant<int, 2>{});
+        else chunk_loop(std::integral_constant<int, 0>{});
+      } else {
+        chunk_loop(std::integral_constant<int, 0>{});
       }
       tl_mark(1);
       consumed_total += nchunks - kres;
@@ -525,7 +641,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
       // the stage is read again by the column phase: it is free only once every warp is past this
       // point, which the NEXT chunk's barrier (or the one below for the last chunk) certifies
       v2_consumer_barrier<NT>();
-      if (tid == 0) issue_next();
+      if (tid == 0) issue_next(std::integral_constant<int, 0>{});
     }
     consumed_total += nchunks;
     ++sweep_no;
@@ -612,41 +728,62 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   if (p.timeline && b == 0 && tid == 0) { tl[16] = ~0ull; tl[17] = 0ull; }
 
   SkLoop L;
-  int cur = 0;
   sweep(false, true, nullptr);
   if (compact) {
     // the 3-byte rows were written through the generic proxy; the bulk copies read them through the async
     // proxy.  Each slab is written and read by its own CTA only, so a CTA barrier suffices.
     asm volatile("fence.proxy.async.global;" ::: "memory");
+    // (the narrow rows' staging words are shared memory the re-carved ring's bulk copies overwrite)
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     // The fp32 ring is drained (no 3-byte chunk is issued before this point): re-carve its memory into the 3-byte
-    // ring and the resident chunks behind it, each stage and chunk R rows of ldc bytes.  The resident run sits in
+    // ring and the resident chunks behind it, each stage and chunk R rows of qp bytes.  The resident run sits in
     // the middle of the slab: there the ring's copies are in flight while the consumers read it, so HBM stays busy.
     // (At either end of a sweep the ring is already full, and every CTA would read its resident chunks at the same
     // time while HBM idles.)
+    // A slab whose chunks are all narrow carves at the narrow row pitch (more resident chunks); otherwise every stage
+    // and resident chunk keeps the 3-byte pitch and a narrow chunk fills the front of its rows.
+    int n_narrow = 0;
+    if constexpr (KG == 4)
+      for (int w = 0; w < kV2MaskWords; ++w) n_narrow += __popc(nmask[w]);
+    const uint32_t ldc = (uint32_t)p.ldc;
+    const int qm = n_narrow == 0 ? 0 : n_narrow == nchunks ? 1 : 2;
+    const uint32_t qp = qm == 1 ? kV2NarrowRow : ldc;
     S = kV2QStages;
     full = bars + 8;
     c_st = 0; c_par = 0; p_st = 0;
-    kres = min(kres_max, nchunks);
+    kres = max(0, min(qbytes / (int)(R * qp) - kV2QStages, nchunks));
     rlo = (nchunks - kres) / 2;
     if (tid == 0) {
-      const uint32_t ldc = (uint32_t)p.ldc;
+      qmode = qm;  // read by the sweeps after the grid barrier below
       if (kres > 0) {
         const int rows = min(nrows - rlo * R, kres * R);
-        v2_mbar_expect_tx(res_full, (uint32_t)rows * ldc);
+        uint32_t bytes = 0;
+        for (int r = 0; r < rows; ++r) bytes += chunk_narrow(rlo + r / R) ? kV2NarrowRow : ldc;
+        v2_mbar_expect_tx(res_full, bytes);
         for (int r = 0; r < rows; ++r)
-          v2_bulk_load(reinterpret_cast<unsigned char*>(stages) + ((size_t)S * R + r) * ldc,
-                       p.mq + (int64_t)(r_begin + rlo * R + r) * ldc, ldc, res_full);
+          v2_bulk_load(reinterpret_cast<unsigned char*>(stages) + ((size_t)S * R + r) * qp,
+                       p.mq + (int64_t)(r_begin + rlo * R + r) * ldc,
+                       chunk_narrow(rlo + r / R) ? kV2NarrowRow : ldc, res_full);
       }
       if (l2_end >= 0) {  // the first streamed chunks of the slab, as many as the fp32 share's bytes
-        const int l2c = (int)(p.l2_resident_frac * (float)nchunks * (4.f * (float)n1) / (float)ldc);
+        const int l2c = (int)(p.l2_resident_frac * (float)nchunks * (4.f * (float)n1) / (float)qp);
         l2_end = min(nchunks, l2c <= rlo ? l2c : l2c + kres);
       }
-      if (kres < nchunks)
-        while (issued < consumed_total + S) issue_next();
+      if (kres < nchunks) {
+        if (qm == 1) while (issued < consumed_total + S) issue_next(std::integral_constant<int, 1>{});
+        else if (qm == 2) while (issued < consumed_total + S) issue_next(std::integral_constant<int, 2>{});
+        else while (issued < consumed_total + S) issue_next(std::integral_constant<int, 0>{});
+      }
     }
   }
   grid.sync();
+  if constexpr (KG == 4)
+    if (compact && tid == 0) {  // CTA 0 cleared the count (sk_ring_init) before the barrier above
+      int n_narrow = 0;
+      for (int w = 0; w < kV2MaskWords; ++w) n_narrow += __popc(nmask[w]);
+      if (n_narrow) atomicAdd(p.n_narrow, n_narrow);
+    }
   combine(nullptr, v_work[0], nullptr);
   grid.sync();
 
@@ -654,6 +791,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
     const SkStep st = sk_step(p, it);
     tl_now = p.timeline && it == 50 && tid == 0;
     tl_mark(0);
+    const int cur = it & 1;  // v_work[cur] holds the current v (every iteration that goes on flips it)
     sweep(true, st.do_col, v_work[cur]);
     L.iters = it + 1;
     if (!st.do_col) break;
@@ -666,7 +804,6 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
     tl_mark(5);
     if (st.check && sk_check_stops(L, p, it)) break;
     if (st.last) break;
-    cur ^= 1;
   }
 
   // ---- drain speculative prefetches so no bulk copy is in flight when the CTA exits ----
@@ -679,7 +816,7 @@ __global__ void __launch_bounds__(NT, 1) sinkhorn_v2_kernel(const SkParams p, in
   }
 
   // kernel variant: 4 = factored on the 3-byte stream, 3 = factored, 2 = log-domain
-  sk_finish(p, L, v_work[cur], kLn2d, 0, compact ? 4 : fact ? 3 : 2);
+  sk_finish(p, L, v_work[(L.iters - 1) & 1], kLn2d, 0, compact ? 4 : fact ? 3 : 2);  // the iteration that stopped
 }
 
 template <int NT, int KG, int R>
@@ -705,22 +842,25 @@ static int v2_launch_t(SkParams& p, cudaStream_t s) {
   int grid = sm_count();
   if (grid > p.n0) grid = p.n0;
   if (grid > kV2MaxGrid) return 1;  // more partials per column than the combine holds in registers
-  // the 3-byte stream re-carves the prologue's ring: kV2QStages stages, then as many resident chunks as fit (no
-  // more than the longest slab has)
+  // the 3-byte stream re-carves the prologue's ring into kV2QStages stages and as many resident chunks as fit (no
+  // more than the longest slab has).  Where chunks may be narrow the kernel sizes the run from their widths, so it
+  // gets the whole budget.
   size_t ring = (size_t)S * stage_bytes;
-  int kres_max = 0;
-  if (p.mq != nullptr) {
+  if (p.ldn != 0) {
+    ring = budget - head;
+  } else if (p.mq != nullptr) {
     const size_t qchunk = (size_t)R * p.ldc;
     const int slab_chunks = ((p.n0 + grid - 1) / grid + R - 1) / R;
-    kres_max = std::max(0, std::min(slab_chunks, (int)((budget - head) / qchunk) - kV2QStages));
+    const int kres_max = std::max(0, std::min(slab_chunks, (int)((budget - head) / qchunk) - kV2QStages));
     ring = std::max(ring, (size_t)(kV2QStages + kres_max) * qchunk);
   }
+  const int qbytes = (int)ring;
   const size_t smem = ring + head;
   CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 0;
   CFM_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, NT, smem));
   if (per_sm < 1) return 1;
-  void* args[] = {(void*)&p, (void*)&S, (void*)&kres_max};
+  void* args[] = {(void*)&p, (void*)&S, (void*)&qbytes};
   CFM_CUDA_OK(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(NT), args, smem, s));
   note_launches(1);
   return CFM_OK;
@@ -757,6 +897,11 @@ int sinkhorn_v2_launch(SkParams& p, cudaStream_t s) {
   p.l2_resident_frac = !streams ? 0.f : l2frac >= 0.f ? l2frac : fminf(1.f, kSkResidentShare * (float)l2 / (float)m_bytes);
   // one 512-thread CTA per SM
   const int kg = (p.n1p / 4 + 511) / 512;
+  // 22-bit chunks where the kernel packs 16 entries per thread (KG = 4) into a row shorter than the 3-byte one
+  // (n1 > 7509); CFM_SK_Q24=1 keeps every chunk at 3 bytes (a cross-check: both give the same bits)
+  static int q24 = -1;
+  if (q24 < 0) { const char* e = getenv("CFM_SK_Q24"); q24 = e && atoi(e) != 0 ? 1 : 0; }
+  p.ldn = kg > 2 && !q24 && p.mq != nullptr && kV2NarrowRow < p.ldc ? (int)kV2NarrowRow : 0;
   if (kg <= 1) return v2_launch_t<512, 1, 8>(p, s);
   if (kg <= 2) return v2_launch_t<512, 2, 4>(p, s);
   return v2_launch_t<512, 4, 2>(p, s);

@@ -4,8 +4,10 @@ the C5 8192 x 8192 d = 128 shard: reg 0.05, normalised cost, 100 iterations, CUD
 (4 = factored sweep on the 3-byte cost stream, 3 = factored on fp32 M).  Bytes are what the variant reads and
 writes of M (part of each sweep comes from the L2, so the HBM fraction is an upper bound of the DRAM share):
     fp32 sweeps:    (iterations + 1) x n0 x n1 x 4
-    3-byte stream:  n0 x n1 x 4 (fp32 prologue) + n0 x ldc (the copy, written once) + iterations x n0 x ldc,
-                    ldc = align16(3 n1)
+    3-byte stream:  n0 x n1 x 4 (fp32 prologue) + C (the copy, written once) + iterations x C,
+                    C = (n0 - nr) x ldc + nr x 22528, ldc = align16(3 n1), nr = rows of the chunks the solve wrote at
+                    22 bits (512 threads x 44 bytes per row; from the count the kernel leaves at workspace byte 288,
+                    0 for a package without 22-bit chunks; 2 rows per chunk, so an upper bound when some are wide)
 --root DIR runs the package found in DIR (e.g. another checkout, for old/new comparisons); --dump DIR saves
 log_u, log_v and the 8192 drawn index pairs of one seeded C2 coupling."""
 import argparse
@@ -44,6 +46,8 @@ for name, n0, n1, d in CONFIGS:
         cp = s._solve_sinkhorn(M, cmax, n0, n1, 0.05, True, bufs=bufs)
     torch.cuda.synchronize()
     ms = []
+    # the count of 22-bit chunks: a package that does not write it leaves the cleared bytes at 0
+    bufs["ws_sk"][288:292].zero_()
     for _ in range(args.reps):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
@@ -54,13 +58,24 @@ for name, n0, n1, d in CONFIGS:
     st = cp.status.cpu().tolist()
     iters = st[1]
     ldc = (3 * n1 + 15) // 16 * 16
+    n_narrow = int(bufs["ws_sk"][288:292].cpu().numpy().view(np.int32)[0])
+    # chunks of the kernel that takes 22-bit chunks (KG = 4, n1 > 4096): 2 rows of one CTA's slab, one CTA per SM
+    # (sk_slab).  Other kernels have other chunk heights, but they write no narrow chunk, so n_narrow = 0 there and
+    # the copy is n0 x ldc whatever `chunks` says.
+    rows_per_chunk = 2 if n1 > 4096 else 4 if n1 > 2048 else 8
+    nslab = min(torch.cuda.get_device_properties(0).multi_processor_count, n0)
+    chunks = sum((n0 // nslab + (1 if b < n0 % nslab else 0) + rows_per_chunk - 1) // rows_per_chunk
+                 for b in range(nslab))
+    nr = n0 if n_narrow == chunks else min(n0, rows_per_chunk * n_narrow)
+    copy = (n0 - nr) * ldc + nr * 512 * 44
     if st[3] == 4:
-        parts = {"fp32_prologue_read": n0 * n1 * 4, "compact_write": n0 * ldc, "compact_reads": iters * n0 * ldc}
+        parts = {"fp32_prologue_read": n0 * n1 * 4, "compact_write": copy, "compact_reads": iters * copy}
     else:
         parts = {"fp32_reads": (iters + 1) * n0 * n1 * 4}
     total = sum(parts.values())
     med = float(np.median(ms))
-    row = {"config": name, "n0": n0, "n1": n1, "d": d, "status": st, "solve_ms_median": med,
+    row = {"config": name, "n0": n0, "n1": n1, "d": d, "status": st, "narrow_chunks": n_narrow, "chunks": chunks,
+           "solve_ms_median": med,
            "solve_ms_min": float(np.min(ms)), "solve_ms_max": float(np.max(ms)), "bytes": parts,
            "bytes_total": total, "bytes_per_s": total / (med * 1e-3), "hbm_fraction": total / (med * 1e-3) / HBM_PEAK}
     rows.append(row)
