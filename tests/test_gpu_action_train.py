@@ -3,12 +3,14 @@ loss of a scalar-action MLP, its input gradient and all eight parameter gradient
 tests/action_oracle.py, the notebook's lines in float64 on the CPU with torch's double backward.
 
 The loss is a difference of terms of size mean(|s0| + |s1| + 1/2 |g_x|^2 + |g_t|), so its error is gated relative to
-that; each parameter gradient relative to its tensor's max-abs.  SELU' and SELU'' jump at 0, so with SELU only rows
+that; each parameter gradient both relative to its tensor's max-abs and entry by entry relative to its own absolute
+scale (tests/train_scale_oracle.py).  SELU' and SELU'' jump at 0, so with SELU only rows
 whose float64 pre-activations at all three evaluation points stay further than _KINK_REL of their magnitude sum from
 the kink are compared (as test_gpu_train.py and test_gpu_action.py gate theirs)."""
 import math
 
 import action_oracle as ao
+import train_scale_oracle as so
 import pytest
 import torch
 
@@ -19,7 +21,8 @@ DEV = "cuda:0"
 gpu = pytest.mark.gpu
 
 BATCHES = [1, 2, 3, 15, 16, 17, 255, 256, 257, 1000, 4096]
-LOSS_REL, GRAD_REL = 2e-6, 2e-5
+LOSS_REL, GRAD_REL = 2e-6, 2e-5  # GRAD_REL: every gradient tensor's error, of its max-abs
+GRAD_ABS = 1.5e-6  # and every entry, of its own absolute scale (tests/train_scale_oracle.py); DESIGN.md 3.13
 _KINK_REL = 1e-5
 
 
@@ -77,19 +80,22 @@ def _device_loss_and_grads(m, xt, t, x0, x1):
 
 
 def _gaps(m, act, xt, t, x0, x1):
-    """(loss error over its scale, worst gradient error over the tensor's max-abs) against the float64 oracle, with
-    b3's gradient checked to be exactly 0."""
+    """(loss error over its scale, worst gradient error over its entry's absolute scale, worst gradient error over
+    the tensor's max-abs) against the float64 oracle, with b3's gradient checked to be exactly 0."""
     loss, grads = _device_loss_and_grads(m, xt, t, x0, x1)
     assert loss.shape == () and loss.dtype == torch.float32 and loss.is_cuda
     rl, rg = ao.action_matching_loss_and_grads(m.state_dict(), m.dim, m.w, xt, t, x0, x1, act)
     scale = ao.loss_scale(ao.make_action(m.state_dict(), m.dim, m.w, act), xt, t, x0, x1)
     lgap = abs(loss.item() - rl.item()) / scale
-    ggap = 0.0
-    for p, g, r in zip(list(m.parameters())[:7], grads[:7], rg[:7]):
+    scales = so.action_grad_scales(m.state_dict(), xt, t, x0, x1, act)
+    ggap = rgap = 0.0
+    for p, g, r, sc in zip(list(m.parameters())[:7], grads[:7], rg[:7], scales[:7]):
         assert g.shape == p.shape and torch.isfinite(g).all()
-        ggap = max(ggap, (g.cpu().double() - r).abs().max().item() / r.abs().max().item())
+        err = (g.cpu().double() - r).abs()
+        ggap = max(ggap, (err / sc.clamp_min(1e-300)).max().item())
+        rgap = max(rgap, err.max().item() / r.abs().max().item())
     assert grads[7].shape == (1,) and grads[7].item() == 0.0
-    return lgap, ggap
+    return lgap, ggap, rgap
 
 
 # ---- every instantiation, every batch-size class -------------------------------------------------------------------
@@ -99,12 +105,13 @@ def _gaps(m, act, xt, t, x0, x1):
 @pytest.mark.parametrize("w", [32, 64])
 def test_loss_and_gradients_match_the_float64_oracle(w, act, dim):
     m = _model(dim, w, act, seed=200 + w + dim)
-    worst = [0.0, 0.0]
+    worst = [0.0, 0.0, 0.0]
     for B in BATCHES:
-        lgap, ggap = _gaps(m, act, *_batch(m, B, seed=B, act=act))
-        assert lgap <= LOSS_REL and ggap <= GRAD_REL, (B, lgap, ggap)
-        worst = [max(worst[0], lgap), max(worst[1], ggap)]
-    print(f"margins w={w} {act} dim={dim}: loss {worst[0]:.2e} grad {worst[1]:.2e}")
+        gaps = _gaps(m, act, *_batch(m, B, seed=B, act=act))
+        assert gaps[0] <= LOSS_REL and gaps[1] <= GRAD_ABS and gaps[2] <= GRAD_REL, (B, gaps)
+        worst = [max(a, b) for a, b in zip(worst, gaps)]
+    print(f"margins w={w} {act} dim={dim}: loss {worst[0]:.2e} grad/abs-scale {worst[1]:.2e} "
+          f"grad/max-abs {worst[2]:.2e}")
 
 
 @gpu
@@ -115,8 +122,8 @@ def test_edge_times_where_the_middle_point_is_an_endpoint(act):
     t[::2], t[1::2] = 0.0, 1.0
     xt = t * x1 + (1 - t) * x0
     keep = _keep(m, act, xt, t, x0, x1)
-    lgap, ggap = _gaps(m, act, xt[keep], t[keep], x0[keep], x1[keep])
-    assert lgap <= LOSS_REL and ggap <= GRAD_REL, (lgap, ggap)
+    lgap, ggap, rgap = _gaps(m, act, xt[keep], t[keep], x0[keep], x1[keep])
+    assert lgap <= LOSS_REL and ggap <= GRAD_ABS and rgap <= GRAD_REL, (lgap, ggap, rgap)
 
 
 @gpu
@@ -241,9 +248,9 @@ def test_twenty_sgd_steps_track_float64_training():
 @pytest.mark.parametrize("act", ["selu", "silu"])
 def test_large_batch_keeps_every_cta_busy(act):
     m = _model(2, 64, act, seed=8)
-    lgap, ggap = _gaps(m, act, *_batch(m, 65536, seed=10, act=act))
-    assert lgap <= LOSS_REL and ggap <= GRAD_REL, (lgap, ggap)
-    print(f"margins B=65536 {act}: loss {lgap:.2e} grad {ggap:.2e}")
+    lgap, ggap, rgap = _gaps(m, act, *_batch(m, 65536, seed=10, act=act))
+    print(f"margins B=65536 {act}: loss {lgap:.2e} grad/abs-scale {ggap:.2e} grad/max-abs {rgap:.2e}")
+    assert lgap <= LOSS_REL and ggap <= GRAD_ABS and rgap <= GRAD_REL, (lgap, ggap, rgap)
 
 
 @gpu

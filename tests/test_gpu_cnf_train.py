@@ -11,6 +11,7 @@ import torch
 
 import cnf_oracle as co
 import cnf_train_oracle as cto
+import train_scale_oracle as so
 from oracle import vector_field as vf
 
 import cfm_b200
@@ -19,6 +20,7 @@ from cfm_b200 import _ffi
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 KERNEL_GATE = 2e-5  # of each gradient tensor's max-abs, kernel at the device states against float64
+ENTRY_GATE = 2e-6   # and of each entry's own absolute scale (tests/train_scale_oracle.py)
 E2E_GATE = 5e-6     # the tutorial's cell against float64 autograd through the float64 trajectory
 SGD_GATE = 5e-6     # parameters after 20 SGD steps against float64 training
 BATCHES = [1, 2, 3, 15, 16, 17, 255, 256, 257, 4096]
@@ -51,6 +53,11 @@ def _largest_batch(dim, w):
     return lo
 
 
+def _entry_errors(got, ref, scales):
+    return [((g.double().cpu() - r.cpu()).abs() / s.cpu().clamp_min(1e-300)).max().item()
+            for g, r, s in zip(got, ref, scales)]
+
+
 def _rel_errors(got, ref):
     return [(g.double() - r).abs().max().item() / max(r.abs().max().item(), 1e-30) for g, r in zip(got, ref)]
 
@@ -70,7 +77,9 @@ def _kernel_case(m, act, B, n, direction, seed):
     params = list(m.parameters())
     got = torch.autograd.grad(traj, params + [z], G)
     ref_p, ref_z = cto.restated_backward(state, traj.detach(), span, G, act, h32=True)
-    return _rel_errors(got, list(ref_p) + [ref_z])
+    sc_p, sc_z = so.cnf_grad_scales(state, traj.detach(), span, G, act)
+    ref = list(ref_p) + [ref_z]
+    return _entry_errors(got, ref, list(sc_p) + [sc_z]), _rel_errors(got, ref)
 
 
 @pytest.mark.parametrize("act", ["selu", "silu"])
@@ -78,15 +87,15 @@ def _kernel_case(m, act, B, n, direction, seed):
 @pytest.mark.parametrize("w", [32, 64])
 def test_backward_kernel_against_the_float64_adjoint_at_the_device_states(w, dim, act):
     m = _mlp(dim, w, act, seed=10 * dim + w)
-    worst = 0.0
+    worst = [0.0, 0.0]
     for i, B in enumerate(BATCHES + [_largest_batch(dim, w)]):
         n, direction = SPANS[i % len(SPANS)]
         if B > 4096:
             n = 2 + i % 2
-        errs = _kernel_case(m, act, B, n, direction, seed=i)
-        worst = max(worst, max(errs))
-        assert max(errs) <= KERNEL_GATE, (B, n, direction, errs)
-    print(f"ERR kernel w={w} dim={dim} act={act} worst={worst:.3e}")
+        errs, rel = _kernel_case(m, act, B, n, direction, seed=i)
+        worst = [max(worst[0], max(errs)), max(worst[1], max(rel))]
+        assert max(errs) <= ENTRY_GATE and max(rel) <= KERNEL_GATE, (B, n, direction, errs, rel)
+    print(f"ERR kernel w={w} dim={dim} act={act} worst grad/abs-scale {worst[0]:.3e} grad/max-abs {worst[1]:.3e}")
 
 
 def _moons(n, g, noise=0.1):
