@@ -32,7 +32,13 @@ class RkState(C.Structure):
                 ("err_acc", C.c_double)]
 
 
-_p, _i, _i64, _f, _d, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double, C.c_size_t
+class SdeState(C.Structure):
+    """Mirror of ``cfm_sde_state`` (include/cfm_b200.h)."""
+    _fields_ = [("seed", C.c_uint64), ("traj", C.c_void_p), ("increments", C.c_void_p), ("n", C.c_int32),
+                ("n_steps", C.c_int32), ("t", C.c_float), ("ticket", C.c_uint32)]
+
+
+_p, _i, _i64, _f, _d, _sz =C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol include/cfm_b200.h declares
 SIGNATURES = {
@@ -85,7 +91,11 @@ SIGNATURES = {
     "cfm_sde_small_supported": (_i, [_i64, _i, _i]),
     "cfm_sde_small_euler_f32": (_i, [_p, _p, _i, _i, _i, _f, _p, _i64, _p, _i, _p, _p, _p, _i, C.c_uint64, _p, _p,
                                      _p]),
-    "cfm_mlp_small_train_supported": (_i, [_i64, _i, _i, _i]),
+    "cfm_sde_tc_supported": (_i, [_i, _i, _i]),
+    "cfm_mlp_pair_forward_split_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _f, _i, _p, _p, _p, _sz, _p]),
+    "cfm_sde_tc_init": (_i, [_p, _p, _p, _p, _p, _p, _p, C.c_uint64, _p, _i, _i, _i, _p]),
+    "cfm_sde_tc_euler_step": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _f, _i, _i, _p]),
+    "cfm_mlp_small_train_supported":(_i, [_i64, _i, _i, _i]),
     "cfm_mlp_small_train_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
     "cfm_mlp_small_mse_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),
     "cfm_mlp_small_action_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),

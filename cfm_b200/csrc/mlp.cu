@@ -159,3 +159,16 @@ extern "C" int cfm_mlp_forward_split_gated_f32(const void* prepared, const void*
   return mlp_tc_forward(h, prepared, nullptr, x_hi, x_lo, batch, t_dev, t_host, act, y, workspace,
                         workspace_bytes, skip_if_nonzero, (cudaStream_t)stream);
 }
+
+extern "C" int cfm_mlp_pair_forward_split_f32(const void* prepared_a, const void* prepared_b, const void* x_hi,
+                                              const void* x_lo, int batch, int dim, int w, int out_dim,
+                                              int time_varying, const float* t_dev, float t_host, int act, float* y_a,
+                                              float* y_b, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "cfm_mlp_pair_forward_split_f32";
+  CFM_REQUIRE(prepared_a && prepared_b && x_hi && x_lo && y_a && y_b && workspace, "%s: null pointer", what);
+  CFM_REQUIRE(act == CFM_ACT_SELU || act == CFM_ACT_SILU, "%s: unknown activation %d", what, act);
+  CFM_REQUIRE(mlp_tc_supported(batch, dim, w, out_dim) != 0, "%s: shape not supported by the tensor-core path", what);
+  const MlpBlobHeader h = mlp_layout(dim, w, out_dim, time_varying ? 1 : 0);
+  return mlp_tc_pair_forward(h, prepared_a, prepared_b, x_hi, x_lo, batch, t_dev, t_host, act, y_a, y_b, workspace,
+                             workspace_bytes, (cudaStream_t)stream);
+}

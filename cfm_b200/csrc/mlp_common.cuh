@@ -17,6 +17,11 @@ size_t mlp_tc_workspace_bytes(int batch, int dim, int w, int out_dim);
 int mlp_tc_forward(const MlpBlobHeader& h, const void* blob, const float* x, const void* x_hi,
                    const void* x_lo, int batch, const float* t_dev, float t_host, int act, float* y, void* ws,
                    size_t ws_bytes, const int32_t* skip, cudaStream_t s);
+// two weight blobs of one shape on the same (x_hi, x_lo): y_a = net_a(x), y_b = net_b(x); ws holds two
+// mlp_tc_workspace_bytes halves
+int mlp_tc_pair_forward(const MlpBlobHeader& h, const void* blob_a, const void* blob_b, const void* x_hi,
+                        const void* x_lo, int batch, const float* t_dev, float t_host, int act, float* y_a,
+                        float* y_b, void* ws, size_t ws_bytes, cudaStream_t s);
 
 static inline MlpBlobHeader mlp_layout(int dim, int w, int out_dim, int tv) {
   MlpBlobHeader h;

@@ -42,11 +42,11 @@
 // All three fields share one integrator body (ode_small_body): the staging, Euler, Hairer's initial step, the dopri5
 // stages, the grid sums, the controller, FSAL and the checkpoint writes.
 #include <cooperative_groups.h>
-#include <curand_philox4x32_x.h>
 
 #include "mlp_small.cuh"
 #include "rk_control.cuh"
 #include "rk_tableau.h"
+#include "sde_common.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -875,21 +875,7 @@ __host__ __device__ inline SdePlan sde_small_plan(int dim, int w, int nwarps, in
   return s;
 }
 
-// Standard normal of (step n, row r, column c): one Philox4x32-10 block per 4 columns, 24-bit uniforms in (0, 1),
-// Box-Muller on (u0, u1) for columns 4q, 4q + 1 and on (u2, u3) for 4q + 2, 4q + 3.  Depends on nothing else.
-__device__ __forceinline__ float sde_normal(uint64_t seed, int n, int64_t r, int c) {
-  const uint4 x = curand_Philox4x32_10(
-      make_uint4((unsigned)(c >> 2), (unsigned)(uint64_t)r, (unsigned)((uint64_t)r >> 32), (unsigned)n),
-      make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
-  const bool hi = c & 2;
-  const unsigned xa = hi ? x.z : x.x, xb = hi ? x.w : x.y;
-  const float ua = __fmaf_rn((float)(xa >> 8), 0x1p-24f, 0x1p-25f);  // exact: 24-bit integer * 2^-24 + 2^-25
-  const float ub = __fmaf_rn((float)(xb >> 8), 0x1p-24f, 0x1p-25f);
-  float s, co;
-  sincospif(2.f * ub, &s, &co);
-  return sqrtf(-2.f * logf(ua)) * ((c & 1) ? s : co);
-}
-
+// dW of the device stream: sde_normal (sde_common.cuh), shared with the tensor-core SDE step (sde_tc.cu)
 template <int U, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) sde_small_kernel(const SdeSmallParams p) {
   constexpr int W = 32 * U;

@@ -236,7 +236,8 @@ class SDE(torch.nn.Module):
 
     ``f`` and ``g`` are the notebooks' plain-PyTorch bodies, so they run on any device and under autograd.  Under
     ``torch.no_grad()`` on CUDA, ``cfm_b200.sdeint`` integrates an SDE whose two nets are ``MLP(time_varying=True)``
-    of one shape in a single kernel instead (cfm_b200/sde.py)."""
+    of one shape on the device instead (cfm_b200/sde.py): small nets in a single kernel, wide nets in the tensor-core
+    class with one launch of both nets' forward and one step kernel per step."""
     noise_type = "diagonal"
     sde_type = "ito"
 

@@ -7,8 +7,16 @@
 (examples/2D_tutorials/SF2M_tutorial.ipynb cell 5, examples/single_cell/single-cell_example.ipynb cell 16).  torchsde
 is an un-vendored dependency; its fixed-step Euler (the step grid, the update and the linear interpolation onto
 ``ts``) is restated in oracle/sde.py and implemented here: the host tabulates the step grid and the output
-interpolation once per ``(ts, dt)``, and ONE kernel (csrc/ode_small.cu, ``sde_small_kernel``) takes every step, both
-MLP evaluations per step, the noise and the output writes.
+interpolation once per ``(ts, dt)``.  Two classes of nets run on the device:
+
+* small nets (w in {32, 64}, both weight sets and the per-row state in shared memory; the 2-D and single-cell
+  tutorials): ONE kernel (csrc/ode_small.cu, ``sde_small_kernel``) takes every step, both MLP evaluations per step,
+  the noise and the output writes;
+* wide nets in the tensor-core class (B >= 128, dim >= 32, dim and w multiples of 8; e.g. the MNIST notebook's
+  ``MLP(784, w=256)``): per step, ONE launch of both nets' fused fp16x3 forward on the state's operand pair
+  (csrc/mlp_h3.cu; per-layer launches for other widths) and ONE elementwise step kernel (csrc/sde_tc.cu).  The step
+  index, time and pointers live in a device struct, so the step is captured once as a CUDA graph and replayed for
+  the whole trajectory, with no host round trip.
 
 Only the SF2M shape is accelerated: a ``cfm_b200.SDE`` whose drift and score are ``cfm_b200.MLP(time_varying=True)``
 of one shape, a CUDA ``(B, D)`` state and ``method="euler"``.  Anything else raises -- there is no eager fallback.
@@ -16,7 +24,8 @@ of one shape, a CUDA ``(B, D)`` state and ``method="euler"``.  Anything else rai
 Noise: torchsde's BrownianInterval stream is not reproduced.  Without ``bm`` the kernel draws its own increments
 from a counter-based generator (Philox4x32-10 + Box-Muller, keyed by one 63-bit seed taken from torch's default CPU
 generator per call), so ``torch.manual_seed`` reproduces a trajectory and the noise of a row does not depend on the
-batch size or the launch shape.  With ``bm`` (a torchsde-style callable ``bm(ta, tb)``) the increments are the
+batch size, the launch shape or the class: a given (seed, step, row, column) draws the same increment in both.
+With ``bm`` (a torchsde-style callable ``bm(ta, tb)``) the increments are the
 caller's, read from device memory.
 """
 import ctypes as C
@@ -29,6 +38,9 @@ from .models import MLP, SDE
 
 _MAX_TABLES = 16
 _tables = {}  # (ts dtype, ts bytes, dt, device) -> (grid, out_begin, out_a, out_b, grid as a CPU tensor in ts's dtype)
+_MAX_PLANS = 4
+_plans = {}   # tensor-core class: plan key (see _tc_plan) -> buffers and the captured step graph
+_EAGER = False  # tests: enqueue every step of the tensor-core class eagerly instead of replaying the captured graph
 
 
 def _refuse_options(method, adaptive, logqp, unsupported):
@@ -130,7 +142,8 @@ def sdeint(sde, y0, ts, bm=None, method=None, dt=1e-3, adaptive=False, logqp=Fal
     ``MLP(time_varying=True)`` nets.  Returns ``ys`` of shape (len(ts), B, D), fp32, on y0's device.
 
     ``bm``: optional callable ``bm(ta, tb) -> (B, D)`` Brownian increment, called once per step in order with 0-d
-    tensors in ts's dtype on ts's device.  Without it the kernel draws the increments itself (module docstring)."""
+    tensors in ts's dtype on ts's device.  Without it the kernels draw the increments themselves (module docstring).
+    Nets in neither class (module docstring) raise ``NotImplementedError``."""
     _refuse_options(method, adaptive, logqp, unsupported)
     drift, score = _nets(sde)
     if not torch.is_tensor(y0) or not y0.is_cuda:
@@ -152,15 +165,18 @@ def sdeint(sde, y0, ts, bm=None, method=None, dt=1e-3, adaptive=False, logqp=Fal
     if not (dt > 0 and np.isfinite(dt)):
         raise ValueError(f"sdeint: dt must be positive and finite; got {dt}")
     L = _ffi.lib()
-    if not L.cfm_sde_small_supported(B, D, drift.w):
+    small = bool(L.cfm_sde_small_supported(B, D, drift.w))
+    if not small and not (B < 2**31 and L.cfm_sde_tc_supported(B, D, drift.w)):
         raise NotImplementedError(
             f"sdeint: no SDE kernel for B={B}, dim={D}, w={drift.w}: it takes cfm_b200.SDE with drift and score "
-            "cfm_b200.MLP(time_varying=True) of w in {32, 64} whose two weight sets and per-row state fit in shared "
-            "memory")
+            "cfm_b200.MLP(time_varying=True) either of w in {32, 64} whose two weight sets and per-row state fit in "
+            "shared memory (one kernel), or in the tensor-core class: B >= 128, dim >= 32, dim and w multiples of 8, "
+            "w >= 32")
     dev = y0.device
-    pd, psc = _weights(drift, dev), _weights(score, dev)
+    pd, psc = (_weights(drift, dev), _weights(score, dev)) if small else (None, None)
     with torch.cuda.device(dev):
-        grid, out_begin, out_a, out_b, grid_host = _tables_for(ts_host, dt, dev)
+        tables = _tables_for(ts_host, dt, dev)
+        grid, out_begin, out_a, out_b, grid_host = tables
         n_steps = grid.numel() - 1
         inc, seed = None, 0
         if bm is None:
@@ -176,6 +192,9 @@ def sdeint(sde, y0, ts, bm=None, method=None, dt=1e-3, adaptive=False, logqp=Fal
             inc = torch.stack(incs).contiguous()
         x0 = y0.detach().float().contiguous()
         ys = torch.empty((ts.numel(), B, D), dtype=torch.float32, device=dev)
+        if not small:
+            _tc_euler(sde, drift, score, x0, tables, seed, inc, ys)
+            return ys
         arr = C.c_void_p * 8  # host arrays of the 8 device pointers of each net
         _ffi.check(L.cfm_sde_small_euler_f32(
             arr(*[p.data_ptr() for p in pd]), arr(*[p.data_ptr() for p in psc]), D, drift.w, drift.act,
@@ -183,3 +202,77 @@ def sdeint(sde, y0, ts, bm=None, method=None, dt=1e-3, adaptive=False, logqp=Fal
             _ffi.ptr(out_b), ts.numel(), seed, _ffi.ptr(inc), _ffi.ptr(ys), _ffi.stream_ptr(dev)),
             "cfm_sde_small_euler_f32")
     return ys
+
+
+# ---- tensor-core class ------------------------------------------------------------------------------------------------
+def _tc_plan(sde, drift, score, B, D, tables, dev):
+    """Buffers of one (shape, both nets' prepared weights, tables, sigma, device, stream): the state y, the nets'
+    outputs, the operand pair (hi, lo) of y, the device state struct, the pair forward's workspace, and -- once the
+    first step has run eagerly -- the CUDA graph of one step.  The graph holds pointers to these buffers, the prepared
+    weight blobs and the tables only; per-call pointers (trajectory, increments) reach it through the state struct."""
+    L = _ffi.lib()
+    # a net's blob is rebuilt when its weights change in place; a plan keeps its blobs and tables alive, so their
+    # addresses name them for as long as the plan exists
+    blobs = (drift._prepared(True, dev), score._prepared(True, dev))
+    key = (B, D, drift.w, drift.act, float(sde.sigma), tuple(t.data_ptr() for t in blobs + tables[:4]), str(dev),
+           torch.cuda.current_stream(dev).cuda_stream)
+    P = _plans.get(key)
+    if P is not None:
+        return P
+    if len(_plans) >= _MAX_PLANS:
+        _plans.pop(next(iter(_plans)))
+    f32 = dict(dtype=torch.float32, device=dev)
+    st = torch.zeros(C.sizeof(_ffi.SdeState), dtype=torch.uint8, device=dev)
+    P = {"blobs": blobs, "tables": tables, "st": st, "y": torch.empty((B, D), **f32),
+         "d": torch.empty((B, D), **f32), "s": torch.empty((B, D), **f32),
+         "hi": torch.empty((B, D), dtype=torch.float16, device=dev),
+         "lo": torch.empty((B, D), dtype=torch.float16, device=dev),
+         "ws": _ffi.workspace(2 * L.cfm_mlp_workspace_bytes(B, D, drift.w, D, 2), dev),
+         "t_dev": C.c_void_p(st.data_ptr() + _ffi.SdeState.t.offset), "graph": None}
+    _plans[key] = P
+    return P
+
+
+def _tc_enqueue_step(sde, drift, P, B, D, dev):
+    """One Euler-Maruyama step: both nets at (t_n, y_n) in one pair launch, then the step kernel."""
+    L = _ffi.lib()
+    sp = _ffi.stream_ptr(dev)
+    grid, out_begin, out_a, out_b, _ = P["tables"]
+    ws = P["ws"]
+    _ffi.check(L.cfm_mlp_pair_forward_split_f32(
+        _ffi.ptr(P["blobs"][0]), _ffi.ptr(P["blobs"][1]), _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), B, D, drift.w, D, 1,
+        P["t_dev"], 0.0, drift.act, _ffi.ptr(P["d"]), _ffi.ptr(P["s"]), _ffi.ptr(ws), ws.numel(), sp),
+        "cfm_mlp_pair_forward_split_f32")
+    _ffi.check(L.cfm_sde_tc_euler_step(
+        _ffi.ptr(P["st"]), _ffi.ptr(P["y"]), _ffi.ptr(P["d"]), _ffi.ptr(P["s"]), _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]),
+        _ffi.ptr(grid), _ffi.ptr(out_begin), _ffi.ptr(out_a), _ffi.ptr(out_b), float(sde.sigma), B, D, sp),
+        "cfm_sde_tc_euler_step")
+
+
+def _tc_euler(sde, drift, score, x0, tables, seed, inc, ys):
+    """The whole trajectory of the tensor-core class into ``ys``: init, then n_steps replays of the step graph (the
+    first call of a plan runs step 0 eagerly, which loads every kernel, then captures the step)."""
+    L = _ffi.lib()
+    dev = x0.device
+    B, D = x0.shape
+    n_steps = tables[0].numel() - 1
+    P = _tc_plan(sde, drift, score, B, D, tables, dev)
+    if x0.data_ptr() % 16:
+        x0 = x0.clone()
+    _ffi.check(L.cfm_sde_tc_init(
+        _ffi.ptr(P["st"]), _ffi.ptr(x0), _ffi.ptr(P["y"]), _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), _ffi.ptr(ys),
+        _ffi.ptr(inc), seed, _ffi.ptr(tables[0]), n_steps, B, D, _ffi.stream_ptr(dev)), "cfm_sde_tc_init")
+    first = 0
+    if _EAGER or P["graph"] is None:
+        _tc_enqueue_step(sde, drift, P, B, D, dev)
+        first = 1
+        if not _EAGER and n_steps > 1:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                _tc_enqueue_step(sde, drift, P, B, D, dev)
+            P["graph"] = g
+    for _ in range(first, n_steps):
+        if _EAGER:
+            _tc_enqueue_step(sde, drift, P, B, D, dev)
+        else:
+            P["graph"].replay()

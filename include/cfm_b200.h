@@ -368,6 +368,48 @@ int cfm_sde_small_euler_f32(const float* const* drift_host, const float* const* 
                             const int* out_begin, const float* out_a, const float* out_b, int n_out, uint64_t seed,
                             const float* increments, float* traj, void* stream);
 
+/* ---- Schrodinger-bridge SDE sampling for WIDE MLPs, on the tensor cores -------------------------------------------
+ * The same SDE, step grid, output interpolation, update expression and noise stream as cfm_sde_small_euler_f32, for
+ * drift and score nets in the tensor-core class (e.g. the MNIST model MLP(784, w=256, time_varying=True)): a driver
+ * (cfm_b200/sde.py) calls cfm_sde_tc_init once per trajectory and then, per step, cfm_mlp_pair_forward_split_f32 on
+ * (y_hi, y_lo) with t_dev = &state->t followed by cfm_sde_tc_euler_step.  Every per-trajectory value the step needs
+ * lives in the device state, so the two step calls can be captured once and replayed n_steps times.
+ * supported(): exactly cfm_mlp_tc_supported(batch, dim, w, dim): batch >= 128, dim >= 32, dim and w multiples of 8,
+ * w >= 32. */
+typedef struct cfm_sde_state {
+  uint64_t seed;            /* key of the device noise stream                                   */
+  float* traj;              /* [n_out][batch][dim]                                              */
+  const float* increments;  /* nullable: [n_steps][batch][dim] Brownian increments              */
+  int32_t n;                /* next step                                                        */
+  int32_t n_steps;
+  float t;                  /* grid[n]: the time the forward of step n reads                    */
+  uint32_t ticket;          /* CTAs of the running step that are done (0 between steps)         */
+} cfm_sde_state;
+int cfm_sde_tc_supported(int batch, int dim, int w);
+/* Both nets (prepared_a, prepared_b: cfm_mlp_prepare blobs of one shape) on the same fp16x3 operand pair:
+ * y_a = net_a(x), y_b = net_b(x), each with the bits cfm_mlp_forward_split_gated_f32 gives it.  For 256-wide hidden
+ * layers and dim >= 64 this is ONE persistent launch over 2 ceil(batch / 128) slabs (net a's, then net b's);
+ * otherwise the per-layer launches of each net in turn.  workspace: 2 * cfm_mlp_workspace_bytes(batch, dim, w,
+ * out_dim, 2) bytes, 16-byte aligned.  Argument errors are reported before any CUDA call. */
+int cfm_mlp_pair_forward_split_f32(const void* prepared_a, const void* prepared_b, const void* x_hi, const void* x_lo,
+                                   int batch, int dim, int w, int out_dim, int time_varying, const float* t_dev,
+                                   float t_host, int act, float* y_a, float* y_b, void* workspace,
+                                   size_t workspace_bytes, void* stream);
+/* state <- (seed, n = 0, t = grid[0], traj, increments); y = traj[0] = y0 (fp32 [batch][dim]) and (y_hi, y_lo) =
+ * its fp16x3 operand split (fp16 [batch][dim] each, the split cfm_mlp_forward_f32 applies to an fp32 input).  Without
+ * increments the step draws dW = sqrt(h) z with z from the stream of cfm_sde_small_euler_f32: a given (seed, step,
+ * row, column) draws the same z in both classes. */
+int cfm_sde_tc_init(cfm_sde_state* state, const float* y0, float* y, void* y_hi, void* y_lo, float* traj,
+                    const float* increments, uint64_t seed, const float* grid, int n_steps, int batch, int dim,
+                    void* stream);
+/* Step n = state->n: y <- fmaf(h, drift + score, y) + sigma dW with h = grid[n + 1] - grid[n]; writes the outputs
+ * out_begin[n] <= k < out_begin[n + 1] of traj, y and (y_hi, y_lo), then n += 1 and t = grid[n + 1].  drift and
+ * score: [batch][dim] fp32 evaluated at (t, y).  A step enqueued after the last one does nothing.  All arrays
+ * 16-byte aligned; argument errors are reported before any CUDA call. */
+int cfm_sde_tc_euler_step(cfm_sde_state* state, float* y, const float* drift, const float* score, void* y_hi,
+                          void* y_lo, const float* grid, const int* out_begin, const float* out_a, const float* out_b,
+                          float sigma, int batch, int dim, void* stream);
+
 /* ---- training step of small vector-field MLPs: the regression loss and all parameter gradients, ONE launch ------
  * replaces the three lines every training cell of the 2-D tutorials repeats per step
  * (examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb raw lines 166-186, 310-330, 458-479, 602-623;
