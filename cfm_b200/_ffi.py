@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libcfm_b200.so")
 
 FLAG_NONFINITE, FLAG_ZERO_MASS, FLAG_NOT_CONVERGED, FLAG_INFEASIBLE = 1, 2, 4, 8
 ACT_SELU, ACT_SILU = 0, 1
+HUTCH_GAUSSIAN, HUTCH_RADEMACHER = 0, 1
 FLOW_ICFM, FLOW_TARGET, FLOW_SB, FLOW_VP = 0, 1, 2, 3
 
 
@@ -35,6 +36,12 @@ class RkState(C.Structure):
 class SdeState(C.Structure):
     """Mirror of ``cfm_sde_state`` (include/cfm_b200.h)."""
     _fields_ = [("seed", C.c_uint64), ("traj", C.c_void_p), ("increments", C.c_void_p), ("n", C.c_int32),
+                ("n_steps", C.c_int32), ("t", C.c_float), ("ticket", C.c_uint32)]
+
+
+class CnfTcState(C.Structure):
+    """Mirror of ``cfm_cnf_tc_state`` (include/cfm_b200.h)."""
+    _fields_ = [("seed", C.c_uint64), ("traj", C.c_void_p), ("t_span", C.c_void_p), ("n", C.c_int32),
                 ("n_steps", C.c_int32), ("t", C.c_float), ("ticket", C.c_uint32)]
 
 
@@ -95,6 +102,11 @@ SIGNATURES = {
     "cfm_mlp_pair_forward_split_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _f, _i, _p, _p, _p, _sz, _p]),
     "cfm_sde_tc_init": (_i, [_p, _p, _p, _p, _p, _p, _p, C.c_uint64, _p, _i, _i, _i, _p]),
     "cfm_sde_tc_euler_step": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _f, _i, _i, _p]),
+    "cfm_cnf_tc_supported": (_i, [_i, _i, _i]),
+    "cfm_cnf_tc_workspace_bytes": (_sz, [_i, _i, _i]),
+    "cfm_cnf_tc_field_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _p, _sz, _p]),
+    "cfm_cnf_tc_euler_init": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i, C.c_uint64, _i, _i, _p]),
+    "cfm_cnf_tc_euler_step": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _i, _p]),
     "cfm_mlp_small_train_supported":(_i, [_i64, _i, _i, _i]),
     "cfm_mlp_small_train_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
     "cfm_mlp_small_mse_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),

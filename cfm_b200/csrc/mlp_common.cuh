@@ -22,6 +22,15 @@ int mlp_tc_forward(const MlpBlobHeader& h, const void* blob, const float* x, con
 int mlp_tc_pair_forward(const MlpBlobHeader& h, const void* blob_a, const void* blob_b, const void* x_hi,
                         const void* x_lo, int batch, const float* t_dev, float t_host, int act, float* y_a,
                         float* y_b, void* ws, size_t ws_bytes, cudaStream_t s);
+// the tensor-core section of a prepared blob, layer l = 0..3: fp16 weight pair (hi, lo) [rows][ld[l]] (rows scaled by
+// one power of two per layer) and the per-row inverse scale; ld[0] covers W0's x columns only (cnf_tc.cu)
+struct MlpTcWeights {
+  const void* wh[4];
+  const void* wl[4];
+  const float* inv_ws[4];
+  int64_t ld[4];
+};
+MlpTcWeights mlp_tc_weights(const MlpBlobHeader& h, const void* blob);
 
 static inline MlpBlobHeader mlp_layout(int dim, int w, int out_dim, int tv) {
   MlpBlobHeader h;

@@ -1,4 +1,5 @@
-// Brownian increments of the SDE samplers (sde_small_kernel in ode_small.cu, sde_tc.cu): one standard normal per
+// Brownian increments of the SDE samplers (sde_small_kernel in ode_small.cu, sde_tc.cu) and the Hutchinson probes of
+// cnf_tc.cu: one standard normal (or Rademacher sign) per
 // (seed, step n, row r, column c), so a given draw is the same in both kernel classes, at any batch size and launch
 // shape.  One Philox4x32-10 block (counter (c / 4, r lo, r hi, n), key (seed lo, seed hi)) serves 4 columns; 24-bit
 // uniforms in (0, 1); Box-Muller on (u0, u1) for columns 4q, 4q + 1 and on (u2, u3) for 4q + 2, 4q + 3.
@@ -37,6 +38,14 @@ __device__ __forceinline__ float4 sde_normal4(uint64_t seed, int n, int64_t r, i
   sincospif(2.f * sde_uniform(x.w), &s1, &c1);
   const float r0 = sqrtf(-2.f * logf(sde_uniform(x.x))), r1 = sqrtf(-2.f * logf(sde_uniform(x.z)));
   return make_float4(r0 * c0, r0 * s0, r1 * c1, r1 * s1);
+}
+
+// Rademacher signs of columns 4q .. 4q + 3 from the same Philox block: column 4q + i is -1 where the top bit of word i
+// is set and +1 otherwise (the Hutchinson probes of csrc/cnf_tc.cu).
+__device__ __forceinline__ float4 sde_rademacher4(uint64_t seed, int n, int64_t r, int q) {
+  const uint4 x = sde_philox(seed, n, r, q);
+  auto sgn = [](unsigned v) { return (v >> 31) ? -1.f : 1.f; };
+  return make_float4(sgn(x.x), sgn(x.y), sgn(x.z), sgn(x.w));
 }
 
 }  // namespace cfm

@@ -273,7 +273,8 @@ class cnf_wrapper(torch.nn.Module):
     ``likelihood_estimator="exact"`` in one kernel instead (cfm_b200/ode.py).  Under autograd, with
     ``solver="euler"``, w in {32, 64}, dim <= 8 and out_dim == dim, that trajectory is differentiable: ``backward()``
     gives the exact gradient of the computed fp32 Euler trajectory for the MLP's parameters and the initial state in
-    one more kernel (csrc/cnf_train.cu); for dopri5 and other shapes it raises ``NotImplementedError``."""
+    one more kernel (csrc/cnf_train.cu); for dopri5 and other shapes it raises ``NotImplementedError``.  The Hutchinson
+    estimators run on the device for models in the tensor-core class (csrc/cnf_tc.cu), with probes the kernels draw."""
 
     def __init__(self, model, likelihood_estimator="exact"):
         super().__init__()

@@ -17,7 +17,11 @@ Only the hot path the north_star names is accelerated: the vector field must be 
 ``cfm_b200.models.MLP`` (optionally inside ``torch_wrapper``) on a CUDA device; anything else
 raises -- there is no eager fallback.  ``cnf_wrapper(MLP(time_varying=True), "exact")`` is accepted too: its
 state carries the log-density column, and the whole trajectory, trace included, runs in the one-launch kernel
-(csrc/ode_small.cu, CNF variant).  So is ``torch_wrapper(GradModel(MLP(time_varying=True, out_dim=1)))``, the
+(csrc/ode_small.cu, CNF variant).  ``cnf_wrapper(MLP(time_varying=True), "hutch_gaussian" | "hutch_rademacher")``
+is accepted for models in the tensor-core class (B >= 128, dim >= 32, dim and w multiples of 8, w >= 32,
+out_dim == dim; e.g. the MNIST model): Hutchinson's eps . (J eps) with one device-drawn probe per evaluation
+(csrc/cnf_tc.cu), Euler with a captured step or dopri5 on the flat [x, ll] state.  So is
+``torch_wrapper(GradModel(MLP(time_varying=True, out_dim=1)))``, the
 action-matching field grad_x s(t, x) (gradient variant).
 
 A decreasing ``t_span`` is integrated as torchdyn does: dopri5 runs the field f_(s, x) = -f(-s, x) over
@@ -53,16 +57,28 @@ def _unwrap(vf):
 
 
 def _unwrap_cnf(vf):
-    if vf.eps_fn is not None:
-        raise NotImplementedError(
-            f"cnf_wrapper(likelihood_estimator={vf.likelihood_estimator!r}): the Hutchinson estimators draw their "
-            "probe vectors from torch's RNG on every call, which no device stream reproduces; the CUDA path "
-            "provides the exact trace (likelihood_estimator='exact')")
     m = vf.model
     if not isinstance(m, MLP) or not m.time_varying:
         raise TypeError("cfm_b200.NeuralODE accelerates cnf_wrapper(cfm_b200.models.MLP(time_varying=True)); got "
                         f"cnf_wrapper({type(m).__name__})")
     return m
+
+
+_HUTCH = {"hutch_gaussian": _ffi.HUTCH_GAUSSIAN, "hutch_rademacher": _ffi.HUTCH_RADEMACHER}
+
+
+def _hutch_refusal(vf, mlp, x):
+    """Raise unless the Hutchinson field of ``cnf_wrapper(mlp)`` on the state ``x`` runs on the tensor cores.  Decided
+    from the shapes alone, before any device check."""
+    B = x.shape[0] if torch.is_tensor(x) and x.dim() == 2 else 0
+    if not (mlp.out_dim == mlp.dim and mlp.act in (_ffi.ACT_SELU, _ffi.ACT_SILU) and 0 < B < 2**31
+            and _ffi.lib().cfm_cnf_tc_supported(B, mlp.dim, mlp.w)):
+        raise NotImplementedError(
+            f"cnf_wrapper(likelihood_estimator={vf.likelihood_estimator!r}): the Hutchinson estimators run on the "
+            "tensor cores for MLP(dim, w, time_varying=True) with out_dim == dim, SELU or SiLU, in the tensor-core "
+            f"class (B >= 128, dim >= 32, dim and w multiples of 8, w >= 32); got B={B}, dim={mlp.dim}, w={mlp.w}, "
+            f"out_dim={mlp.out_dim}.  For dim <= 8 use likelihood_estimator='exact': the exact trace costs only dim "
+            "tangents there and has no variance")
 
 
 def _grad_model(vf):
@@ -123,6 +139,7 @@ class NeuralODE(torch.nn.Module):
         # the step sequence a single process would take on the full batch.
         self.lockstep = None
         self._plans = {}
+        self._cnf_plans = {}  # Hutchinson Euler: plan key -> buffers and the captured step graph
 
     def forward(self, x, t_span):
         traj = self.trajectory(x, t_span)
@@ -136,6 +153,8 @@ class NeuralODE(torch.nn.Module):
         {32, 64}, dim <= 8, out_dim == dim, SELU or SiLU) ``backward()`` computes the exact gradient of the computed
         fp32 Euler trajectory in one launch, whatever ``sensitivity`` says; outside the class it raises
         ``NotImplementedError`` with the reason.  The forward is the same launch with the same bits either way."""
+        if isinstance(self.vf, cnf_wrapper) and self.vf.eps_fn is not None:
+            _hutch_refusal(self.vf, _unwrap_cnf(self.vf), x)
         if isinstance(self.vf, cnf_wrapper) and torch.is_grad_enabled():
             mlp = _unwrap_cnf(self.vf)
             params = list(mlp.parameters())
@@ -152,6 +171,9 @@ class NeuralODE(torch.nn.Module):
 
     def _cnf_backward_gap(self, mlp, x):
         """Why backward() through this cnf_wrapper trajectory is not implemented, or None when it is."""
+        if self.vf.eps_fn is not None:
+            return (f"gradients through the Hutchinson-estimator trajectory (likelihood_estimator="
+                    f"{self.vf.likelihood_estimator!r}) are not implemented; the device path samples it only")
         if self.solver != "euler":
             return (f"gradients through the adaptive {self.solver} solve are not implemented; use solver='euler'")
         B = x.shape[0] if x.dim() == 2 else 0
@@ -173,12 +195,17 @@ class NeuralODE(torch.nn.Module):
         dev = x.device
         t_span = torch.as_tensor(t_span, dtype=torch.float32)
         reverse = self.solver == "dopri5" and _decreasing(t_span)  # see the module docstring
+        kw = {}
+        if cnf and self.vf.eps_fn is not None:
+            # the Hutchinson probes' seed, one per call from torch's default CPU generator, drawn first: building the
+            # time-reversed net below initialises a module, which draws from the same generator on its first use
+            kw["seed"] = int(torch.randint(0, 2**63 - 1, (), dtype=torch.int64))
         with torch.cuda.device(dev):  # the library launches on the CURRENT device: make it the tensors' one
             if reverse:
                 mlp, t_span = mlp._time_reversed(), -t_span
             run = (self._cnf_trajectory_on if cnf else self._grad_trajectory_on if gm is not None
                    else self._trajectory_on)
-            out = run(mlp, x, t_span, dev)
+            out = run(mlp, x, t_span, dev, **kw)
         if reverse:
             self.stats["t"] = -self.stats["t"]
         return out
@@ -199,7 +226,7 @@ class NeuralODE(torch.nn.Module):
             out = self._dopri5(mlp, x0, t_span.detach().cpu().contiguous())
         return out.reshape(out.shape[0], *shape)
 
-    def _cnf_trajectory_on(self, mlp, x, t_span, dev):
+    def _cnf_trajectory_on(self, mlp, x, t_span, dev, seed=None):
         """cnf_wrapper(mlp, "exact"): the state [x, ll] goes through the CNF variant of the one-launch kernel."""
         if self.lockstep is not None:
             raise NotImplementedError("cnf_wrapper: lock-step sharding is not supported; the exact-likelihood path "
@@ -209,12 +236,82 @@ class NeuralODE(torch.nn.Module):
                              f"column), got {tuple(x.shape)}")
         if t_span.numel() < 2:
             raise ValueError("cnf_wrapper: t_span needs at least two points")
+        if self.vf.eps_fn is not None:
+            _hutch_refusal(self.vf, mlp, x)
+            return self._hutch_trajectory(mlp, x.detach().float().contiguous(), t_span, dev, seed)
         if mlp.out_dim != mlp.dim or not _ffi.lib().cfm_ode_small_cnf_supported(x.shape[0], mlp.dim, mlp.w):
             raise NotImplementedError(
                 f"cnf_wrapper: no exact-likelihood kernel for B={x.shape[0]}, dim={mlp.dim}, w={mlp.w}, "
                 f"out_dim={mlp.out_dim} (it takes w in {{32, 64, 128}}, dim <= 8, out_dim == dim and batches whose "
-                "state fits in shared memory)")
+                "state fits in shared memory); models in the tensor-core class (B >= 128, dim >= 32, dim and w "
+                "multiples of 8, w >= 32) take likelihood_estimator='hutch_gaussian' or 'hutch_rademacher'")
         return self._fused_small(mlp, x.detach().float().contiguous(), t_span.to(dev).contiguous(), cnf=True)
+
+    def _hutch_trajectory(self, mlp, z, t_span, dev, seed):
+        """cnf_wrapper(mlp, "hutch_*") in the tensor-core class (csrc/cnf_tc.cu): the field is [f, eps . (J eps)] with
+        one fresh probe per evaluation, keyed by ``seed`` (drawn by ``_trajectory``)."""
+        est = self.vf.likelihood_estimator
+        if self.solver == "euler":
+            return self._hutch_euler(mlp, z, t_span.to(dev).contiguous(), est, seed)
+        B, D = z.shape[0], mlp.dim
+        flat = torch.cat([z[:, :D].reshape(-1), z[:, D]])  # the x block [B][D], then the ll block [B]
+        return self._dopri5(mlp, flat, t_span.detach().cpu().contiguous(), cnf=(est, seed, B, D))
+
+    def _hutch_euler(self, mlp, z, t_span, est, seed):
+        """Euler over ``t_span`` (fp32 on the device): init, then per step the ten launches of one field evaluation and
+        the step kernel, captured once as a CUDA graph per plan and replayed."""
+        L = _ffi.lib()
+        dev = z.device
+        B, D, n_span = z.shape[0], mlp.dim, t_span.numel()
+        blob = mlp._prepared(True, dev)
+        key = (id(mlp), B, D, str(dev), mlp._weights_key(), blob.data_ptr(), mlp.act, est,
+               torch.cuda.current_stream(dev).cuda_stream)
+        P = self._cnf_plans.get(key)
+        if P is None:
+            self._cnf_plans.clear()  # one live plan: a new shape / new weights retire the old graph
+            f32 = dict(dtype=torch.float32, device=dev)
+            st = torch.zeros(C.sizeof(_ffi.CnfTcState), dtype=torch.uint8, device=dev)
+            P = {"blob": blob, "st": st, "x": torch.empty((B, D), **f32), "ll": torch.empty(B, **f32),
+                 "f": torch.empty((B, D), **f32), "div": torch.empty(B, **f32),
+                 "hi": torch.empty((B, D), dtype=torch.float16, device=dev),
+                 "lo": torch.empty((B, D), dtype=torch.float16, device=dev),
+                 "ws": _ffi.workspace(L.cfm_cnf_tc_workspace_bytes(B, D, mlp.w), dev), "graph": None}
+            self._cnf_plans[key] = P
+        st, ws = P["st"], P["ws"]
+        at = lambda off: C.c_void_p(st.data_ptr() + off)  # noqa: E731
+
+        def step():  # on the current stream, which is the capture stream inside torch.cuda.graph
+            sp = _ffi.stream_ptr(dev)
+            _ffi.check(L.cfm_cnf_tc_field_f32(
+                _ffi.ptr(blob), None, _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), B, D, mlp.w, mlp.act, _HUTCH[est],
+                at(_ffi.CnfTcState.t.offset), at(_ffi.CnfTcState.seed.offset), at(_ffi.CnfTcState.n.offset), 0,
+                _ffi.ptr(P["f"]), _ffi.ptr(P["div"]), _ffi.ptr(ws), ws.numel(), sp), "cfm_cnf_tc_field_f32")
+            _ffi.check(L.cfm_cnf_tc_euler_step(_ffi.ptr(st), _ffi.ptr(P["x"]), _ffi.ptr(P["ll"]), _ffi.ptr(P["f"]),
+                                               _ffi.ptr(P["div"]), _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), B, D, sp),
+                       "cfm_cnf_tc_euler_step")
+
+        traj = torch.empty((n_span, B, D + 1), dtype=torch.float32, device=dev)
+        P["span"] = t_span  # read through the state by every step: kept alive with the plan
+        _ffi.check(L.cfm_cnf_tc_euler_init(_ffi.ptr(st), _ffi.ptr(z), _ffi.ptr(P["x"]), _ffi.ptr(P["ll"]),
+                                           _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), _ffi.ptr(traj), _ffi.ptr(t_span),
+                                           n_span, seed, B, D, _ffi.stream_ptr(dev)), "cfm_cnf_tc_euler_init")
+        first = 0
+        if not self.use_cuda_graph or P["graph"] is None:
+            step()  # (the first call of a plan loads every kernel before the capture)
+            first = 1
+            if self.use_cuda_graph and n_span > 2:
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    step()
+                P["graph"] = g
+        for _ in range(first, n_span - 1):
+            if self.use_cuda_graph:
+                P["graph"].replay()
+            else:
+                step()
+        self.stats = {"nfe": n_span - 1, "accepted": n_span - 1, "rejected": 0,
+                      "graph": self.use_cuda_graph and P["graph"] is not None}
+        return traj
 
     def _grad_trajectory_on(self, mlp, x, t_span, dev):
         """torch_wrapper(GradModel(mlp)): the field grad_x mlp(t, x) through the gradient variant of the one-launch
@@ -294,7 +391,7 @@ class NeuralODE(torch.nn.Module):
                                                 _ffi.ptr(P["xs_hi"]), _ffi.ptr(P["xs_lo"]), _ffi.ptr(P["t_stage"]),
                                                 _ffi.ptr(xs if stage == 6 else None),  # error partial -> xs (free here)
                                                 numel, stage, sp), "cfm_rk_stage_input")
-                mlp.vector_field_split(P["t_stage"], P["xs_hi"], P["xs_lo"], k[stage], skip_flag=P["done_flag"])
+                P["field_split"](P["t_stage"], P["xs_hi"], P["xs_lo"], k[stage], P["done_flag"], stage - 1)
             else:
                 _ffi.check(L.cfm_rk_stage_input(stp, _ffi.ptr(x), _ffi.ptr(k), _ffi.ptr(out), None, None,
                                                 _ffi.ptr(P["t_stage"]), None, numel, stage, sp), "cfm_rk_stage_input")
@@ -307,51 +404,83 @@ class NeuralODE(torch.nn.Module):
         _ffi.check(L.cfm_rk_commit(stp, _ffi.ptr(x), _ffi.ptr(xnew), _ffi.ptr(k), _ffi.ptr(P["traj"]),
                                    numel, sp), "cfm_rk_commit")
 
-    def _plan(self, mlp, B, D, n_span, dev):
-        """Persistent buffers (+ the captured step graph) for one problem shape and weight version."""
-        key = (id(mlp), B, D, n_span, str(dev), mlp._weights_key(), mlp.mlp_algo, mlp.act, self.lockstep is not None)
+    def _plan(self, mlp, B, D, n_span, dev, cnf=None):
+        """Persistent buffers (+ the captured step graph) for one problem shape and weight version.  ``cnf``: the
+        Hutchinson estimator of a cnf_wrapper state, laid out flat as the x block [B][D] followed by the ll block [B]
+        (numel = B (D + 1)); every cfm_rk_* kernel takes that layout unchanged."""
+        key = (id(mlp), B, D, n_span, str(dev), mlp._weights_key(), mlp.mlp_algo, mlp.act, self.lockstep is not None,
+               cnf)
         P = self._plans.get(key)
         if P is not None:
             return P
         self._plans.clear()  # one live plan: a new shape / new weights retire the old graph
         st = torch.zeros(ctypes_sizeof_state(), dtype=torch.uint8, device=dev)
-        P = {"dev": dev, "numel": B * D, "st": st, "stp": _ffi.ptr(st),
-             "x": torch.empty((B, D), dtype=torch.float32, device=dev),
-             "xnew": torch.empty((B, D), dtype=torch.float32, device=dev),
-             "xs": torch.empty((B, D), dtype=torch.float32, device=dev),
-             "k": torch.empty((7, B, D), dtype=torch.float32, device=dev),
-             "traj": torch.empty((n_span, B, D), dtype=torch.float32, device=dev),
+        numel = B * D if cnf is None else B * (D + 1)
+        shape = (B, D) if cnf is None else (numel,)
+        P = {"dev": dev, "numel": numel, "st": st, "stp": _ffi.ptr(st),
+             "x": torch.empty(shape, dtype=torch.float32, device=dev),
+             "xnew": torch.empty(shape, dtype=torch.float32, device=dev),
+             "xs": torch.empty(shape, dtype=torch.float32, device=dev),
+             "k": torch.empty((7, *shape), dtype=torch.float32, device=dev),
+             "traj": torch.empty((n_span, *shape), dtype=torch.float32, device=dev),
              "t_span": torch.empty(n_span, dtype=torch.float32, device=dev),
              "t_stage": torch.zeros(1, dtype=torch.float32, device=dev),
              "scratch": torch.zeros(4, dtype=torch.float64, device=dev),
              "pinned": torch.empty(ctypes_sizeof_state(), dtype=torch.uint8, pin_memory=True),
              "pinned_init": torch.empty(ctypes_sizeof_state(), dtype=torch.uint8, pin_memory=True),
              "t0": torch.zeros(1, dtype=torch.float32, device=dev), "ts_host": None, "init_graph": None,
-             "xs_hi": None, "xs_lo": None, "graph": None, "group": None, "dist": None, "numel_global": B * D}
+             "xs_hi": None, "xs_lo": None, "graph": None, "group": None, "dist": None, "numel_global": numel}
         off = _ffi.RkState.err_acc.offset  # the float64 accumulator inside the device state struct
         P["err_acc"] = st[off:off + 8].view(torch.float64)
         off = _ffi.RkState.done.offset  # int32: non-zero once t has reached t_end
         P["done_flag"] = st[off:off + 4].view(torch.int32)
-        if mlp.tc_path(B):
+        if cnf is not None or mlp.tc_path(B):
             # stage inputs go to the MLP as its fp16x3 tensor-core operand pair (hi, lo), written by the RK kernel
-            P["xs_hi"] = torch.empty((B, D), dtype=torch.float16, device=dev)
-            P["xs_lo"] = torch.empty((B, D), dtype=torch.float16, device=dev)
+            P["xs_hi"] = torch.empty(shape, dtype=torch.float16, device=dev)
+            P["xs_lo"] = torch.empty(shape, dtype=torch.float16, device=dev)
+        if cnf is None:
+            P["field"] = lambda t, x, out, n: mlp.vector_field(t, x, out=out)
+            P["field_split"] = lambda t, hi, lo, out, skip, n: mlp.vector_field_split(t, hi, lo, out, skip_flag=skip)
+        else:
+            self._hutch_fields(mlp, P, B, D, cnf)
         self._plans[key] = P
         return P
+
+    @staticmethod
+    def _hutch_fields(mlp, P, B, D, est):
+        """The plan's field launchers for the flat [x, ll] state: f into the first B D elements of ``out``, div into the
+        last B.  The probe ordinal is the controller's ``nfe`` plus the evaluation's place in the init (0, 1) or the
+        step (stage - 1), read on the device, and the seed is the plan's device word."""
+        L = _ffi.lib()
+        dev = P["dev"]
+        blob = mlp._prepared(True, dev)
+        ws = _ffi.workspace(L.cfm_cnf_tc_workspace_bytes(B, D, mlp.w), dev)
+        P["blob"], P["cnf_ws"] = blob, ws
+        P["seed"] = torch.zeros(1, dtype=torch.int64, device=dev)
+        nfe = C.c_void_p(P["st"].data_ptr() + _ffi.RkState.nfe.offset)
+
+        def field(t, x, out, n, hi=None, lo=None):
+            _ffi.check(L.cfm_cnf_tc_field_f32(
+                _ffi.ptr(blob), _ffi.ptr(x), _ffi.ptr(hi), _ffi.ptr(lo), B, D, mlp.w, mlp.act, _HUTCH[est], _ffi.ptr(t),
+                _ffi.ptr(P["seed"]), nfe, n, _ffi.ptr(out), C.c_void_p(out.data_ptr() + 4 * B * D), _ffi.ptr(ws),
+                ws.numel(), _ffi.stream_ptr(dev)), "cfm_cnf_tc_field_f32")
+
+        P["field"] = field
+        P["field_split"] = lambda t, hi, lo, out, skip, n: field(t, None, out, n, hi, lo)
 
     def _enqueue_init(self, mlp, P, lock):
         """k1 = f(t0, x) and the Hairer initial step (one extra evaluation), enqueued without a host round trip."""
         L = _ffi.lib()
         sp = _ffi.stream_ptr(P["dev"])
         stp, x, xs, k, numel, ng = P["stp"], P["x"], P["xs"], P["k"], P["numel"], P["numel_global"]
-        mlp.vector_field(P["t0"], x, out=k[0])
+        P["field"](P["t0"], x, k[0], 0)
         _ffi.check(L.cfm_rk_init_sums(stp, _ffi.ptr(x), _ffi.ptr(k[0]), None, _ffi.ptr(P["scratch"]), numel, 0, sp),
                    "cfm_rk_init_sums")
         if lock:
             P["dist"].all_reduce(P["scratch"], group=P["group"])
         _ffi.check(L.cfm_rk_init_probe(stp, _ffi.ptr(x), _ffi.ptr(k[0]), _ffi.ptr(xs), _ffi.ptr(P["t_stage"]),
                                        _ffi.ptr(P["scratch"]), numel, ng, sp), "cfm_rk_init_probe")
-        mlp.vector_field(P["t_stage"], xs, out=k[1])
+        P["field"](P["t_stage"], xs, k[1], 1)
         if lock:  # phase 1 adds into scratch[2] only; keep the already-global scratch[0:2] out of the second reduce
             P["scratch"][2:].zero_()
         _ffi.check(L.cfm_rk_init_sums(stp, _ffi.ptr(x), _ffi.ptr(k[0]), _ffi.ptr(k[1]), _ffi.ptr(P["scratch"]),
@@ -361,13 +490,16 @@ class NeuralODE(torch.nn.Module):
         _ffi.check(L.cfm_rk_init_finish(stp, _ffi.ptr(P["t_span"]), _ffi.ptr(P["scratch"]), ng, sp),
                    "cfm_rk_init_finish")
 
-    def _dopri5(self, mlp, x0, ts_host):
-        """``ts_host``: the span as a contiguous fp32 CPU tensor."""
+    def _dopri5(self, mlp, x0, ts_host, cnf=None):
+        """``ts_host``: the span as a contiguous fp32 CPU tensor.  ``cnf``: (estimator, seed, B, D) of a Hutchinson
+        cnf_wrapper state, ``x0`` then being its flat layout (see ``_plan``); the result is (n_span, B, D + 1)."""
         dev = x0.device
-        B, D = x0.shape
+        B, D = x0.shape if cnf is None else cnf[2:]
         numel = x0.numel()
         n_span = ts_host.numel()
-        P = self._plan(mlp, B, D, n_span, dev)
+        P = self._plan(mlp, B, D, n_span, dev, None if cnf is None else cnf[0])
+        if cnf is not None:
+            P["seed"].fill_(cnf[1])
         x, traj, st = P["x"], P["traj"], P["st"]
         x.copy_(x0)
         traj[0].copy_(x0)
@@ -445,7 +577,10 @@ class NeuralODE(torch.nn.Module):
             raise RuntimeError("dopri5: step budget exhausted")
         P["last_steps"] = int(cur.accepted) + int(cur.rejected)
         self.stats = _rk_stats(cur, graph=P["graph"] is not None and not lock, lockstep=lock)
-        return traj.clone()
+        if cnf is None:
+            return traj.clone()
+        n = B * D  # one copy back to the (n_span, B, D + 1) layout
+        return torch.cat([traj[:, :n].view(n_span, B, D), traj[:, n:].view(n_span, B, 1)], 2)
 
 
 class _CnfEulerTrajectory(torch.autograd.Function):

@@ -410,6 +410,50 @@ int cfm_sde_tc_euler_step(cfm_sde_state* state, float* y, const float* drift, co
                           void* y_lo, const float* grid, const int* out_begin, const float* out_a, const float* out_b,
                           float sigma, int batch, int dim, void* stream);
 
+/* ---- Hutchinson log-likelihood of WIDE MLP flows, on the tensor cores --------------------------------------------
+ * replaces the field of cnf_wrapper(model, likelihood_estimator="hutch_gaussian" / "hutch_rademacher")
+ * (examples/2D_tutorials/Maximum_likelihood_CNF_tutorial.ipynb, get_div_and_eps) for MLP(dim, w, time_varying=True)
+ * with out_dim == dim in the tensor-core class: d/dt [x, ll] = [f(t, x), eps . (J eps)], J = df/dx at (t, x), with a
+ * fresh probe eps per evaluation.  Entry (r, c) of probe n is the normal of the SDE noise stream (Philox4x32-10 counter
+ * (c / 4, r lo, r hi, n), key (seed lo, seed hi), Box-Muller) or, for Rademacher, -1 where the top bit of Philox word
+ * c % 4 of the same counter is set and +1 otherwise: a function of (seed, n, r, c) only.
+ * supported(): exactly cfm_mlp_tc_supported(batch, dim, w, dim). */
+#define CFM_HUTCH_GAUSSIAN 0
+#define CFM_HUTCH_RADEMACHER 1
+int cfm_cnf_tc_supported(int batch, int dim, int w);
+size_t cfm_cnf_tc_workspace_bytes(int batch, int dim, int w);
+/* One field evaluation at (t = *t_dev, x) for `batch` rows: f [batch][dim] (row stride dim) and div [batch], fp32,
+ * any 4-byte alignment.  x is given either as fp32 [batch][dim] (x_hi = x_lo = NULL; split here) or as its fp16x3
+ * operand pair (x = NULL), as cfm_rk_stage_input writes it.  The probe ordinal is *ordinal_dev + ordinal_offset and
+ * the seed *seed_dev, both read on the device, so a captured evaluation replays with new values.  prepared: the
+ * cfm_mlp_prepare blob (time_varying = 1, out_dim = dim).  Ten launches: probe (and x split), four primal and four
+ * tangent GEMMs, the fold of the per-chunk float64 partials of eps . (J eps) in a fixed order (the same call gives the
+ * same bits).  x, x_hi, x_lo and the workspace 16-byte aligned; argument errors are reported before any CUDA call. */
+int cfm_cnf_tc_field_f32(const void* prepared, const float* x, const void* x_hi, const void* x_lo, int batch, int dim,
+                         int w, int act, int estimator, const float* t_dev, const uint64_t* seed_dev,
+                         const int32_t* ordinal_dev, int ordinal_offset, float* f, float* div, void* workspace,
+                         size_t workspace_bytes, void* stream);
+/* Euler driver state: step n evaluates the field at (t = t_span[n], x_n) with probe ordinal n (torchdyn's count). */
+typedef struct cfm_cnf_tc_state {
+  uint64_t seed;          /* key of the probe stream                                          */
+  float* traj;            /* [n_span][batch][dim + 1]                                         */
+  const float* t_span;    /* [n_span] fp32                                                    */
+  int32_t n;              /* next step (and the probe ordinal of its evaluation)              */
+  int32_t n_steps;        /* n_span - 1                                                       */
+  float t;                /* t_span[n]: the time the evaluation of step n reads               */
+  uint32_t ticket;        /* CTAs of the running step that are done (0 between steps)         */
+} cfm_cnf_tc_state;
+/* state <- (seed, traj, t_span, n = 0, t = t_span[0]); z0 [batch][dim + 1] -> x [batch][dim], ll [batch], traj[0] and
+ * (x_hi, x_lo), the fp16x3 operand split of x.  x, x_hi, x_lo 16-byte aligned. */
+int cfm_cnf_tc_euler_init(cfm_cnf_tc_state* state, const float* z0, float* x, float* ll, void* x_hi, void* x_lo,
+                          float* traj, const float* t_span, int n_span, uint64_t seed, int batch, int dim,
+                          void* stream);
+/* Step n = state->n with h = (float)((double)t_span[n + 1] - (double)t_span[n]): x <- fmaf(h, f, x),
+ * ll <- fmaf(h, div, ll), traj[n + 1], (x_hi, x_lo); then n += 1, t = t_span[n + 1].  A step enqueued after the last
+ * one does nothing.  x, f, x_hi, x_lo 16-byte aligned. */
+int cfm_cnf_tc_euler_step(cfm_cnf_tc_state* state, float* x, float* ll, const float* f, const float* div, void* x_hi,
+                          void* x_lo, int batch, int dim, void* stream);
+
 /* ---- training step of small vector-field MLPs: the regression loss and all parameter gradients, ONE launch ------
  * replaces the three lines every training cell of the 2-D tutorials repeats per step
  * (examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb raw lines 166-186, 310-330, 458-479, 602-623;
