@@ -173,3 +173,24 @@ def stream_ptr(device=None):
 def workspace(nbytes, device):
     """Scratch bytes from torch's caching allocator (the library never allocates)."""
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
+
+
+def replay_steps(plan, step, n_steps, graph):
+    """Enqueue ``n_steps`` calls of ``step``, which launches one step on the current stream and reads everything that
+    changes from step to step from device memory.  With ``graph``, the first call of a plan runs step 0 eagerly (which
+    loads every kernel), captures one step into ``plan["graph"]`` when more steps follow, and replays it for the rest;
+    later calls replay it for every step.  Without ``graph`` every step is enqueued eagerly."""
+    first = 0
+    if not graph or plan["graph"] is None:
+        step()
+        first = 1
+        if graph and n_steps > 1:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                step()
+            plan["graph"] = g
+    for _ in range(first, n_steps):
+        if graph:
+            plan["graph"].replay()
+        else:
+            step()

@@ -16,8 +16,10 @@
 //             32-column chunk;
 //   fold      div_r = sum of row r's partials in chunk order.
 // No floating-point atomics touch a sum: the same call gives the same bits.  The Euler driver's init and step kernels
-// follow sde_tc.cu: the step index (= the probe ordinal), time, seed and trajectory pointer live in a device struct,
-// so a captured step replays for the whole trajectory.
+// work like sde_tc.cu's: the step index (= the probe ordinal), time, seed and trajectory pointer live in a device
+// struct, so a captured step replays for the whole trajectory.  Shared with sde_tc.cu: the operand split and packing
+// (gemm_h3.cuh), the state's shape rule and step advance (sde_common.cuh) and the launch grid (common.cuh); the GEMMs
+// go through launch_gemm_h3 with this file's kernel entry.
 #include "gemm_h3.cuh"
 #include "mlp_small.cuh"  // act_deriv_fast
 #include "sde_common.cuh"
@@ -48,25 +50,6 @@ CnfWs cnf_ws(int batch, int dim, int w) {
 }
 
 bool cnf_tc_shape(int batch, int dim, int w) { return mlp_tc_supported(batch, dim, w, dim) != 0; }
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-__device__ __forceinline__ uint4 pack8h(const __half (&h)[8]) {
-  return make_uint4((uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
-                    (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16),
-                    (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16),
-                    (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16));
-}
-
-// 4 values -> their saturating (hi, lo) split at quad i
-__device__ __forceinline__ void split4_store(const float4 v, __half* hi, __half* lo, int64_t i) {
-  __half h[4], l[4];
-  split_h3_sat(v.x, h[0], l[0]); split_h3_sat(v.y, h[1], l[1]);
-  split_h3_sat(v.z, h[2], l[2]); split_h3_sat(v.w, h[3], l[3]);
-  reinterpret_cast<uint2*>(hi)[i] = make_uint2((uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
-                                               (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16));
-  reinterpret_cast<uint2*>(lo)[i] = make_uint2((uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16),
-                                               (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16));
-}
 
 // one row's 32 values -> (hi, lo) at hi/lo + [0, 32) (16-byte aligned) or, for a partial chunk, [0, n)
 __device__ __forceinline__ void split_row32(const float (&v)[32], __half* hi, __half* lo, bool full, int n) {
@@ -136,7 +119,7 @@ struct CnfPrimalEpi {
     }
     if (act < 0) {
       float* base = f + (int64_t)row0 * ldo + col0;
-      if (full && (ldo & 3) == 0 && aligned16_dev(base)) {
+      if (full && (ldo & 3) == 0 && aligned16(base)) {
         tc_store_chunk32(tile, v, base, ldo, n0 - row0, lane);
       } else if (row < n0) {
 #pragma unroll
@@ -165,9 +148,6 @@ struct CnfPrimalEpi {
     split_row32(v, out_hi + (int64_t)row * ldo + col0, out_lo + (int64_t)row * ldo + col0, full, n1 - col0);
   }
   __device__ __forceinline__ void finish(int) {}
-  __device__ static __forceinline__ bool aligned16_dev(const float* p) {
-    return (reinterpret_cast<uintptr_t>(p) & 15) == 0;
-  }
 };
 
 // tangent layer: J_l u = acc / s_W; hidden: u' = act'(pre) * J_l u, split; output layer: float64 partial of
@@ -227,34 +207,6 @@ cnf_gemm_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constan
   gemm_wg_body<H3Scheme, Epi, false>(map_ah, map_al, map_bh, map_bl, p, epi);
 }
 
-// launch_gemm_h3 / launch_gemm_wg with cnf_gemm_kernel: D[m, n] = sum_k A[m, k] B[n, k], grid = min(tiles, SMs)
-template <class Epi>
-int launch_cnf_gemm(const __half* ah, const __half* al, int n0, int64_t lda, const __half* bh, const __half* bl, int n1,
-                    int64_t ldb, int d, Epi epi, cudaStream_t s) {
-  CUtensorMap mah, mal, mbh, mbl;
-  int rc;
-  if ((rc = tc_make_map_f16(&mah, ah, n0, d, lda, kTM)) != CFM_OK) return rc;
-  if ((rc = tc_make_map_f16(&mal, al, n0, d, lda, kTM)) != CFM_OK) return rc;
-  if ((rc = tc_make_map_f16(&mbh, bh, n1, d, ldb, kTN)) != CFM_OK) return rc;
-  if ((rc = tc_make_map_f16(&mbl, bl, n1, d, ldb, kTN)) != CFM_OK) return rc;
-  TcShape p;
-  p.n0 = n0; p.n1 = n1; p.d = d;
-  p.tiles_m = (n0 + kTM - 1) / kTM;
-  p.tiles_n = (n1 + kTN - 1) / kTN;
-  int grid = p.tiles_m * p.tiles_n;
-  if (grid > sm_count()) grid = sm_count();
-  static bool attr_set = false;  // per Epi
-  if (!attr_set) {
-    CFM_CUDA_OK(cudaFuncSetAttribute(cnf_gemm_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)kWgSmemBytes));
-    attr_set = true;
-  }
-  cnf_gemm_kernel<Epi><<<grid, kWgThreads, kWgSmemBytes, s>>>(mah, mal, mbh, mbl, p, epi);
-  note_launches(1);
-  CFM_CUDA_OK(cudaGetLastError());
-  return CFM_OK;
-}
-
 // div_r = sum over chunks k of parts[r][k], in k order
 __global__ void __launch_bounds__(256) cnf_fold_kernel(const double* __restrict__ parts, int nchunk,
                                                        float* __restrict__ div, int batch) {
@@ -263,13 +215,6 @@ __global__ void __launch_bounds__(256) cnf_fold_kernel(const double* __restrict_
   double s = 0.0;
   for (int k = 0; k < nchunk; ++k) s += parts[(int64_t)r * nchunk + k];
   div[r] = (float)s;
-}
-
-int ew_grid(int64_t n) {
-  int64_t blocks = (n + 255) / 256;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  return (int)(blocks < 1 ? 1 : blocks);
 }
 
 // ---- Euler driver -------------------------------------------------------------------------------------------------
@@ -324,16 +269,7 @@ cnf_euler_step_kernel(cfm_cnf_tc_state* st, float4* __restrict__ x, float* __res
     ll[r] = v;
     out[r * ld + ld - 1] = v;
   }
-  // every CTA read n above; the last one to get here moves the state on to step n + 1
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(&st->ticket, 1u) == gridDim.x - 1) {
-      st->n = n + 1;
-      st->t = t1;
-      st->ticket = 0u;
-    }
-  }
+  step_advance(st, n, t1);
 }
 
 }  // namespace
@@ -401,12 +337,14 @@ extern "C" int cfm_cnf_tc_field_f32(const void* prepared, const float* x, const 
     CnfPrimalEpi pe;
     pe.bias = F(boff[l]); pe.inv_ws = W.inv_ws[l]; pe.tcol = l == 0 ? F(h.off_w0t) : nullptr; pe.t_dev = t_dev;
     pe.act = l < 3 ? act : -1; pe.dact = dact; pe.out_hi = oph; pe.out_lo = opl; pe.f = f; pe.ldo = n1; pe.t = 0.f;
-    if ((rc = launch_cnf_gemm(ph, pl, batch, (int64_t)K, wh, wl, n1, W.ld[l], K, pe, s)) != CFM_OK) return rc;
+    rc = launch_gemm_h3<CnfPrimalEpi, cnf_gemm_kernel<CnfPrimalEpi>>(ph, pl, batch, K, wh, wl, n1, W.ld[l], K, pe, s);
+    if (rc != CFM_OK) return rc;
     CnfTangentEpi te;
     te.inv_ws = W.inv_ws[l]; te.dact = dact; te.out_hi = oth; te.out_lo = otl; te.ldo = n1;
     te.eps = l == 3 ? reinterpret_cast<const float*>(ws + P.eps) : nullptr;
     te.parts = reinterpret_cast<double*>(ws + P.parts); te.nchunk = P.nchunk;
-    if ((rc = launch_cnf_gemm(th, tl, batch, (int64_t)K, wh, wl, n1, W.ld[l], K, te, s)) != CFM_OK) return rc;
+    rc = launch_gemm_h3<CnfTangentEpi, cnf_gemm_kernel<CnfTangentEpi>>(th, tl, batch, K, wh, wl, n1, W.ld[l], K, te, s);
+    if (rc != CFM_OK) return rc;
     ph = oph; pl = opl; th = oth; tl = otl;
   }
   cnf_fold_kernel<<<(batch + 255) / 256, 256, 0, s>>>(reinterpret_cast<const double*>(ws + P.parts), P.nchunk, div,
@@ -422,8 +360,7 @@ extern "C" int cfm_cnf_tc_euler_init(cfm_cnf_tc_state* state, const float* z0, f
   const char* what = "cfm_cnf_tc_euler_init";
   CFM_REQUIRE(state && z0 && x && ll && x_hi && x_lo && traj && t_span, "%s: null pointer", what);
   CFM_REQUIRE(n_span >= 2, "%s: n_span must be >= 2 (got %d)", what, n_span);
-  CFM_REQUIRE(batch >= 128 && dim >= 32 && dim % 8 == 0,
-              "%s: unsupported shape B=%d dim=%d (B >= 128, dim >= 32, dim %% 8 == 0)", what, batch, dim);
+  if (const int rc = tc_state_shape(what, batch, dim)) return rc;
   CFM_REQUIRE(aligned16(x) && aligned16(x_hi) && aligned16(x_lo) && (reinterpret_cast<uintptr_t>(state) & 7) == 0,
               "%s: x, x_hi and x_lo must be 16-byte aligned, the state 8-byte aligned", what);
   const int64_t n4 = (int64_t)batch * dim / 4;
@@ -439,8 +376,7 @@ extern "C" int cfm_cnf_tc_euler_step(cfm_cnf_tc_state* state, float* x, float* l
                                      void* x_hi, void* x_lo, int batch, int dim, void* stream) {
   const char* what = "cfm_cnf_tc_euler_step";
   CFM_REQUIRE(state && x && ll && f && div && x_hi && x_lo, "%s: null pointer", what);
-  CFM_REQUIRE(batch >= 128 && dim >= 32 && dim % 8 == 0,
-              "%s: unsupported shape B=%d dim=%d (B >= 128, dim >= 32, dim %% 8 == 0)", what, batch, dim);
+  if (const int rc = tc_state_shape(what, batch, dim)) return rc;
   CFM_REQUIRE(aligned16(x) && aligned16(f) && aligned16(x_hi) && aligned16(x_lo) &&
                   (reinterpret_cast<uintptr_t>(state) & 7) == 0,
               "%s: x, f, x_hi and x_lo must be 16-byte aligned, the state 8-byte aligned", what);

@@ -37,6 +37,16 @@ size_t l2_bytes();          // cached cudaDevAttrL2CacheSize of the current devi
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// grid of a 256-thread grid-stride elementwise kernel over n items: one item per thread, at most 8 CTAs per SM
+inline int ew_grid(int64_t n) {
+  const int64_t blocks = (n + 255) / 256, cap = (int64_t)sm_count() * 8;
+  return (int)(blocks > cap ? cap : blocks < 1 ? 1 : blocks);
+}
+
+__host__ __device__ __forceinline__ bool aligned16(const void* p) {
+  return (reinterpret_cast<uintptr_t>(p) & 15) == 0;
+}
+
 // ---- device helpers ------------------------------------------------------------
 #ifdef __CUDACC__
 constexpr float kLog2e = 1.4426950408889634f;

@@ -76,13 +76,35 @@ __device__ __forceinline__ void split_h3_sat_x2(float v0, float v1, uint32_t& hi
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo2) : "f"(r1), "f"(r0));
 }
 
+// 4 or 8 fp16 -> one 8- or 16-byte word, element 0 in the low half of the first 32 bits
+__device__ __forceinline__ uint2 pack4h(const __half (&h)[4]) {
+  return make_uint2((uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
+                    (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16));
+}
+__device__ __forceinline__ uint4 pack8h(const __half (&h)[8]) {
+  return make_uint4((uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
+                    (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16),
+                    (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16),
+                    (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16));
+}
+
+// 4 values -> their saturating (hi, lo) split at quad i of hi and lo
+__device__ __forceinline__ void split4_store(const float4 v, __half* hi, __half* lo, int64_t i) {
+  __half h[4], l[4];
+  split_h3_sat(v.x, h[0], l[0]); split_h3_sat(v.y, h[1], l[1]);
+  split_h3_sat(v.z, h[2], l[2]); split_h3_sat(v.w, h[3], l[3]);
+  reinterpret_cast<uint2*>(hi)[i] = pack4h(h);
+  reinterpret_cast<uint2*>(lo)[i] = pack4h(l);
+}
+
 // ---- host side -------------------------------------------------------------------------------------
 // (rows, d) fp16 row-major (row stride ld halves, ld % 8 == 0) -> box of (box_rows x 64 halves), 128B swizzle,
 // zero fill outside [0, d) x [0, rows).  Descriptors are cached by (base, shape): see sqdist_h3.cu.
 int tc_make_map_f16(CUtensorMap* m, const __half* base, int rows, int d, int64_t ld, int box_rows);
 
-// Epilogue functor interface: see gemm_tc.cuh (acc = acc0 + acc1 * 2^-11)
-template <class Epi>
+// Epilogue functor interface: see gemm_tc.cuh (acc = acc0 + acc1 * 2^-11).  `kern`: the kernel entry (see
+// launch_gemm_wg).
+template <class Epi, auto kern = wg_entry<H3Scheme, Epi>()>
 inline int launch_gemm_h3(const __half* ah, const __half* al, int n0, int64_t lda, const __half* bh,
                           const __half* bl, int n1, int64_t ldb, int d, Epi epi, cudaStream_t s) {
   CUtensorMap mah, mal, mbh, mbl;
@@ -91,7 +113,7 @@ inline int launch_gemm_h3(const __half* ah, const __half* al, int n0, int64_t ld
   if ((rc = tc_make_map_f16(&mal, al, n0, d, lda, kTM)) != CFM_OK) return rc;
   if ((rc = tc_make_map_f16(&mbh, bh, n1, d, ldb, kTN)) != CFM_OK) return rc;
   if ((rc = tc_make_map_f16(&mbl, bl, n1, d, ldb, kTN)) != CFM_OK) return rc;
-  return launch_gemm_wg<H3Scheme>(mah, mal, mbh, mbl, n0, n1, d, epi, s);
+  return launch_gemm_wg<H3Scheme, Epi, kern>(mah, mal, mbh, mbl, n0, n1, d, epi, s);
 }
 
 }  // namespace cfm

@@ -299,8 +299,16 @@ template <class Epi, class = void> struct wg_declares_split_k : std::false_type 
 template <class Epi> struct wg_declares_split_k<Epi, std::void_t<decltype(Epi::kSplitK)>> : std::true_type {};
 
 // ---- host side -------------------------------------------------------------------------------------
-// launch of gemm_wg_kernel on prepared tensor maps (grid = min(tiles, SMs))
+// the default kernel entry of an epilogue: gemm_wg_splitk_kernel if it declares kSplitK, gemm_wg_kernel otherwise
 template <class Scheme, class Epi>
+constexpr auto wg_entry() {
+  if constexpr (wg_declares_split_k<Epi>::value) return gemm_wg_splitk_kernel<Scheme, Epi>;
+  else return gemm_wg_kernel<Scheme, Epi>;
+}
+
+// launch of the kernel entry `kern` on prepared tensor maps (grid = min(tiles, SMs)).  A file passes an entry of its own
+// to keep its GEMMs apart from the instantiations other files' tests pin.
+template <class Scheme, class Epi, auto kern = wg_entry<Scheme, Epi>()>
 inline int launch_gemm_wg(const CUtensorMap& mah, const CUtensorMap& mal, const CUtensorMap& mbh,
                           const CUtensorMap& mbl, int n0, int n1, int d, Epi epi, cudaStream_t s) {
   TcShape p;
@@ -308,14 +316,10 @@ inline int launch_gemm_wg(const CUtensorMap& mah, const CUtensorMap& mal, const 
   p.tiles_m = (n0 + kTM - 1) / kTM;
   p.tiles_n = (n1 + kTN - 1) / kTN;
   int grid = p.tiles_m * p.tiles_n;
-  auto kern = [] {
-    if constexpr (wg_declares_split_k<Epi>::value) return gemm_wg_splitk_kernel<Scheme, Epi>;
-    else return gemm_wg_kernel<Scheme, Epi>;
-  }();
   if constexpr (wg_declares_split_k<Epi>::value) {
     if constexpr (Epi::kSplitK) grid *= epi.k_slices;
   }
-  static bool attr_set = false;  // per (Scheme, Epi) instantiation
+  static bool attr_set = false;  // per kernel instantiation
   if (!attr_set) {
     CFM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgSmemBytes));
     attr_set = true;

@@ -11,15 +11,15 @@
 //
 // Buffers (fp32, numel = B*D each): x, xnew, xs (stage input), k[0..6] contiguous (k1..k7).
 // All elementwise kernels are HBM-bound: float4 accesses, grid = 4 CTAs/SM, grid-stride loops.
-#include <cuda_fp16.h>
-
-#include "common.cuh"
+#include "gemm_h3.cuh"  // pack4h
 #include "rk_control.cuh"
 #include "rk_tableau.h"
 
 namespace cfm {
 
-// fp16x3 operand split (gemm_h3.cuh): hi = fp16(v), lo = fp16((v - hi) * 2^11), saturating
+// fp16x3 operand split (gemm_h3.cuh): hi = fp16(v), lo = fp16((v - hi) * 2^11), saturating.  Not split_h3_sat: the
+// clamp before __float2half_rn turns a NaN into -65504, where cvt.rn.satfinite keeps it NaN, so the two differ on a
+// NaN state.
 __device__ __forceinline__ void rk_split_h3(float v, __half& hi, __half& lo) {
   const float c = fminf(fmaxf(v, -65504.f), 65504.f);
   hi = __float2half_rn(c);
@@ -49,7 +49,7 @@ __device__ __forceinline__ float4 rk_ld_pol(const float4* ptr, uint64_t pol) {
   return v;
 }
 
-static inline int ew_grid(int64_t numel) {
+static inline int rk_ew_grid(int64_t numel) {
   int64_t blocks = (numel / 4 + 255) / 256 + 1;
   const int64_t cap = (int64_t)sm_count() * 8;
   return (int)(blocks < cap ? blocks : cap);
@@ -133,12 +133,8 @@ rk_stage_input_kernel(const cfm_rk_state* __restrict__ st, const float* __restri
         __half h[4], l[4];
         rk_split_h3(v[u].x, h[0], l[0]); rk_split_h3(v[u].y, h[1], l[1]);
         rk_split_h3(v[u].z, h[2], l[2]); rk_split_h3(v[u].w, h[3], l[3]);
-        reinterpret_cast<uint2*>(out_hi)[i] = make_uint2(
-            (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
-            (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16));
-        reinterpret_cast<uint2*>(out_lo)[i] = make_uint2(
-            (uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16),
-            (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16));
+        reinterpret_cast<uint2*>(out_hi)[i] = pack4h(h);
+        reinterpret_cast<uint2*>(out_lo)[i] = pack4h(l);
       }
     }
   }
@@ -309,7 +305,7 @@ extern "C" int cfm_rk_stage_input(const cfm_rk_state* st, const float* x, const 
 extern "C" int cfm_rk_error_norm(cfm_rk_state* st, const float* x, const float* xnew, const float* k,
                                  const float* err_partial, int64_t numel, void* stream) {
   RK_CHECK(st && x && xnew && k && numel > 0);
-  rk_error_norm_kernel<<<ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, xnew, k, err_partial, numel); ::cfm::note_launches(1);
+  rk_error_norm_kernel<<<rk_ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, xnew, k, err_partial, numel); ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
 }
@@ -322,7 +318,7 @@ extern "C" int cfm_rk_control(cfm_rk_state* st, const float* t_span, int64_t num
 extern "C" int cfm_rk_commit(const cfm_rk_state* st, float* x, const float* xnew, float* k, float* traj,
                              int64_t numel, void* stream) {
   RK_CHECK(st && x && xnew && k && traj && numel > 0);
-  rk_commit_kernel<<<ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, xnew, k, traj, numel); ::cfm::note_launches(1);
+  rk_commit_kernel<<<rk_ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, xnew, k, traj, numel); ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
 }
@@ -335,9 +331,9 @@ extern "C" int cfm_rk_init_sums(const cfm_rk_state* st, const float* x, const fl
   cudaStream_t s = (cudaStream_t)stream;
   if (phase == 0) {
     CFM_CUDA_OK(cudaMemsetAsync(scratch, 0, 4 * sizeof(double), s));
-    rk_init_reduce_a<<<ew_grid(numel), 256, 0, s>>>(st, x, f0, scratch, numel); ::cfm::note_launches(1);
+    rk_init_reduce_a<<<rk_ew_grid(numel), 256, 0, s>>>(st, x, f0, scratch, numel); ::cfm::note_launches(1);
   } else {
-    rk_init_reduce_b<<<ew_grid(numel), 256, 0, s>>>(st, x, f0, f1, scratch, numel); ::cfm::note_launches(1);
+    rk_init_reduce_b<<<rk_ew_grid(numel), 256, 0, s>>>(st, x, f0, f1, scratch, numel); ::cfm::note_launches(1);
   }
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
@@ -346,7 +342,7 @@ extern "C" int cfm_rk_init_probe(cfm_rk_state* st, const float* x, const float* 
                                  float* t_stage, const double* scratch, int64_t numel, int64_t numel_global,
                                  void* stream) {
   RK_CHECK(st && x && f0 && x_probe && scratch && numel > 0 && numel_global >= numel);
-  rk_init_probe<<<ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, f0, x_probe, t_stage, scratch, numel,
+  rk_init_probe<<<rk_ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(st, x, f0, x_probe, t_stage, scratch, numel,
                                                                  numel_global); ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
@@ -361,7 +357,7 @@ extern "C" int cfm_rk_init_finish(cfm_rk_state* st, const float* t_span, const d
 extern "C" int cfm_axpy_f32(const float* x, const float* k, float h, float* x_out, int64_t numel,
                             void* stream) {
   RK_CHECK(x && k && x_out && numel > 0);
-  axpy_kernel<<<ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(x, k, h, x_out, numel); ::cfm::note_launches(1);
+  axpy_kernel<<<rk_ew_grid(numel), 256, 0, (cudaStream_t)stream>>>(x, k, h, x_out, numel); ::cfm::note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;
 }

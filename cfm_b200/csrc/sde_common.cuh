@@ -3,9 +3,12 @@
 // (seed, step n, row r, column c), so a given draw is the same in both kernel classes, at any batch size and launch
 // shape.  One Philox4x32-10 block (counter (c / 4, r lo, r hi, n), key (seed lo, seed hi)) serves 4 columns; 24-bit
 // uniforms in (0, 1); Box-Muller on (u0, u1) for columns 4q, 4q + 1 and on (u2, u3) for 4q + 2, 4q + 3.
+// Also the step state the Euler drivers of sde_tc.cu and cnf_tc.cu share (cfm_sde_state, cfm_cnf_tc_state).
 #pragma once
 #include <curand_philox4x32_x.h>
 #include <stdint.h>
+
+#include "common.cuh"
 
 namespace cfm {
 
@@ -46,6 +49,30 @@ __device__ __forceinline__ float4 sde_rademacher4(uint64_t seed, int n, int64_t 
   const uint4 x = sde_philox(seed, n, r, q);
   auto sgn = [](unsigned v) { return (v >> 31) ? -1.f : 1.f; };
   return make_float4(sgn(x.x), sgn(x.y), sgn(x.z), sgn(x.w));
+}
+
+// ---- step state of the tensor-core Euler drivers ------------------------------------------------------------------
+// The state side of the tensor-core class (mlp_tc_supported(batch, dim, w, dim) without w): CFM_OK, or CFM_ERR_ARG
+// with the error naming the entry point `what`.
+inline int tc_state_shape(const char* what, int batch, int dim) {
+  CFM_REQUIRE(batch >= 128 && dim >= 32 && dim % 8 == 0,
+              "%s: unsupported shape B=%d dim=%d (B >= 128, dim >= 32, dim %% 8 == 0)", what, batch, dim);
+  return CFM_OK;
+}
+
+// End of a step kernel that ran step n: the CTA that finishes last moves the state on to step n + 1 at time t_next.
+// Every CTA must have read st->n before it gets here.  State: a struct with int n, float t and unsigned ticket.
+template <class State>
+__device__ __forceinline__ void step_advance(State* st, int n, float t_next) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&st->ticket, 1u) == gridDim.x - 1) {
+      st->n = n + 1;
+      st->t = t_next;
+      st->ticket = 0u;
+    }
+  }
 }
 
 }  // namespace cfm

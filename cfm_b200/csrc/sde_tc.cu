@@ -8,22 +8,14 @@
 //   * advances the step index and the time the next forward reads.
 // Everything a step needs from one call to the next -- step index, time, seed, trajectory and increment pointers --
 // lives in a device struct (cfm_sde_state) written by the init kernel, so one captured step replays for the whole
-// trajectory with no host round trip and no per-call pointer in the graph.
+// trajectory with no host round trip and no per-call pointer in the graph.  Shared with cnf_tc.cu: the operand split
+// (split4_store, gemm_h3.cuh), the state's shape rule and step advance (sde_common.cuh) and the launch grid
+// (common.cuh).
 #include "gemm_h3.cuh"
 #include "mlp_common.cuh"
 #include "sde_common.cuh"
 
 namespace cfm {
-
-__device__ __forceinline__ void split4_store(const float4 v, __half* hi, __half* lo, int64_t i) {
-  __half h[4], l[4];
-  split_h3_sat(v.x, h[0], l[0]); split_h3_sat(v.y, h[1], l[1]);
-  split_h3_sat(v.z, h[2], l[2]); split_h3_sat(v.w, h[3], l[3]);
-  reinterpret_cast<uint2*>(hi)[i] = make_uint2((uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
-                                               (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16));
-  reinterpret_cast<uint2*>(lo)[i] = make_uint2((uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16),
-                                               (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16));
-}
 
 // state <- (seed, step 0, t = grid[0], traj, increments); y = traj[0] = y0 and y0's operand split
 __global__ void sde_tc_init_kernel(cfm_sde_state* __restrict__ st, const float4* __restrict__ y0, float4* __restrict__ y,
@@ -83,28 +75,8 @@ sde_tc_step_kernel(cfm_sde_state* st, float4* __restrict__ y, const float4* __re
     y[i] = y1;
     split4_store(y1, hi, lo, i);
   }
-  // every CTA read n above; the last one to get here moves the state on to step n + 1
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(&st->ticket, 1u) == gridDim.x - 1) {
-      st->n = n + 1;
-      st->t = grid[n + 1];
-      st->ticket = 0u;
-    }
-  }
+  step_advance(st, n, grid[n + 1]);
 }
-
-static int sde_ew_grid(int64_t n4) {
-  int64_t blocks = (n4 + 255) / 256;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  return (int)(blocks < cap ? blocks : cap);
-}
-
-// the state side of the tensor-core class (cfm_mlp_tc_supported(batch, dim, w, dim) without w)
-static bool sde_tc_shape(int batch, int dim) { return batch >= 128 && dim >= 32 && dim % 8 == 0; }
-
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace cfm
 
@@ -118,13 +90,12 @@ extern "C" int cfm_sde_tc_init(cfm_sde_state* state, const float* y0, float* y, 
   const char* what = "cfm_sde_tc_init";
   CFM_REQUIRE(state && y0 && y && y_hi && y_lo && traj && grid, "%s: null pointer", what);
   CFM_REQUIRE(n_steps >= 1, "%s: n_steps must be >= 1 (got %d)", what, n_steps);
-  CFM_REQUIRE(sde_tc_shape(batch, dim), "%s: unsupported shape B=%d dim=%d (B >= 128, dim >= 32, dim %% 8 == 0)", what,
-              batch, dim);
+  if (const int rc = tc_state_shape(what, batch, dim)) return rc;
   CFM_REQUIRE(aligned16(y0) && aligned16(y) && aligned16(y_hi) && aligned16(y_lo) && aligned16(traj) &&
                   aligned16(increments) && (reinterpret_cast<uintptr_t>(state) & 7) == 0,
               "%s: y0, y, y_hi, y_lo, traj and increments must be 16-byte aligned, the state 8-byte aligned", what);
   const int64_t n4 = (int64_t)batch * dim / 4;
-  sde_tc_init_kernel<<<sde_ew_grid(n4), 256, 0, (cudaStream_t)stream>>>(
+  sde_tc_init_kernel<<<ew_grid(n4), 256, 0, (cudaStream_t)stream>>>(
       state, reinterpret_cast<const float4*>(y0), reinterpret_cast<float4*>(y), reinterpret_cast<__half*>(y_hi),
       reinterpret_cast<__half*>(y_lo), traj, increments, seed, grid, n_steps, n4);
   note_launches(1);
@@ -139,13 +110,12 @@ extern "C" int cfm_sde_tc_euler_step(cfm_sde_state* state, float* y, const float
   const char* what = "cfm_sde_tc_euler_step";
   CFM_REQUIRE(state && y && drift && score && y_hi && y_lo && grid && out_begin && out_a && out_b, "%s: null pointer",
               what);
-  CFM_REQUIRE(sde_tc_shape(batch, dim), "%s: unsupported shape B=%d dim=%d (B >= 128, dim >= 32, dim %% 8 == 0)", what,
-              batch, dim);
+  if (const int rc = tc_state_shape(what, batch, dim)) return rc;
   CFM_REQUIRE(aligned16(y) && aligned16(drift) && aligned16(score) && aligned16(y_hi) && aligned16(y_lo) &&
                   (reinterpret_cast<uintptr_t>(state) & 7) == 0,
               "%s: y, drift, score, y_hi and y_lo must be 16-byte aligned, the state 8-byte aligned", what);
   const int64_t n4 = (int64_t)batch * dim / 4;
-  sde_tc_step_kernel<<<sde_ew_grid(n4), 256, 0, (cudaStream_t)stream>>>(
+  sde_tc_step_kernel<<<ew_grid(n4), 256, 0, (cudaStream_t)stream>>>(
       state, reinterpret_cast<float4*>(y), reinterpret_cast<const float4*>(drift),
       reinterpret_cast<const float4*>(score), reinterpret_cast<__half*>(y_hi), reinterpret_cast<__half*>(y_lo), grid,
       out_begin, out_a, out_b, sigma, dim / 4, n4);

@@ -115,12 +115,8 @@ __global__ void prep_rows_h3_kernel(const float* __restrict__ X, int rows, int d
     __half hh[4], ll[4];
     split_h3(v.x * sc, hh[0], ll[0]); split_h3(v.y * sc, hh[1], ll[1]);
     split_h3(v.z * sc, hh[2], ll[2]); split_h3(v.w * sc, hh[3], ll[3]);
-    *reinterpret_cast<uint2*>(h + 4 * k) = make_uint2(
-        (uint32_t)__half_as_ushort(hh[0]) | ((uint32_t)__half_as_ushort(hh[1]) << 16),
-        (uint32_t)__half_as_ushort(hh[2]) | ((uint32_t)__half_as_ushort(hh[3]) << 16));
-    *reinterpret_cast<uint2*>(l + 4 * k) = make_uint2(
-        (uint32_t)__half_as_ushort(ll[0]) | ((uint32_t)__half_as_ushort(ll[1]) << 16),
-        (uint32_t)__half_as_ushort(ll[2]) | ((uint32_t)__half_as_ushort(ll[3]) << 16));
+    *reinterpret_cast<uint2*>(h + 4 * k) = pack4h(hh);
+    *reinterpret_cast<uint2*>(l + 4 * k) = pack4h(ll);
   }
 }
 

@@ -255,8 +255,8 @@ struct TcHiddenEpi {
         __half hh[8], ll[8];
 #pragma unroll
         for (int c = 0; c < 8; ++c) split_h3_sat(o[8 * g + c], hh[c], ll[c]);
-        *reinterpret_cast<uint4*>(ph + 8 * g) = pack8(hh);
-        *reinterpret_cast<uint4*>(pl + 8 * g) = pack8(ll);
+        *reinterpret_cast<uint4*>(ph + 8 * g) = pack8h(hh);
+        *reinterpret_cast<uint4*>(pl + 8 * g) = pack8h(ll);
       }
     }
 #pragma unroll
@@ -274,13 +274,6 @@ struct TcHiddenEpi {
     }
   }
   __device__ __forceinline__ void finish(int) {}
-  // pack 8 fp16 into one 16-byte word
-  __device__ static __forceinline__ uint4 pack8(const __half (&h)[8]) {
-    return make_uint4((uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16),
-                      (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16),
-                      (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16),
-                      (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16));
-  }
 };
 
 // layer 3: y = acc / s_W + b, d = s y - target; loss partial sum d^2 per 32 x 32 chunk (float64), e_3 = r = s d
@@ -573,8 +566,7 @@ extern "C" int cfm_mlp_tc_mse_grad_f32(const float* W0, const float* b0, const f
   }
   int64_t total = 0;
   for (int k = 0; k < fp.njobs; ++k) total += (int64_t)fp.j[k].n0 * fp.j[k].n1;
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, (int64_t)sm_count() * 8));
-  tc_fold_kernel<<<grid, 256, 0, s>>>(fp);
+  tc_fold_kernel<<<ew_grid(total), 256, 0, s>>>(fp);
   note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;

@@ -43,6 +43,16 @@ class MLP(torch.nn.Module):
         return tuple((p.data_ptr(), p._version) for lin in self._linears()
                      for p in (lin.weight, lin.bias))
 
+    def _device_params(self, device):
+        """The eight parameters (weight and bias of each Linear in order), detached and contiguous, for the kernels."""
+        ps = []
+        for lin in self._linears():
+            for p in (lin.weight, lin.bias):
+                if p.device != device or p.dtype != torch.float32:
+                    raise _ffi.CfmLibraryError("MLP parameters must be fp32 on the input's CUDA device")
+                ps.append(p.detach().contiguous())
+        return ps
+
     def _prepared(self, split_t, device):
         """Device blob for the kernels.  ``split_t``: treat the last input column as the shared
         scalar time (torch_wrapper path) instead of a data column."""
@@ -57,12 +67,7 @@ class MLP(torch.nn.Module):
         tv = 1 if split_t else 0
         nbytes = L.cfm_mlp_prepared_bytes(dim, self.w, self.out_dim, tv)
         blob = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        ps = []
-        for lin in self._linears():
-            for p in (lin.weight, lin.bias):
-                if p.device != device or p.dtype != torch.float32:
-                    raise _ffi.CfmLibraryError("MLP parameters must be fp32 on the input's CUDA device")
-                ps.append(p.detach().contiguous())
+        ps = self._device_params(device)
         with torch.cuda.device(device):
             _ffi.check(L.cfm_mlp_prepare(*[_ffi.ptr(p) for p in ps], dim, self.w, self.out_dim, tv,
                                          _ffi.ptr(blob), nbytes, _ffi.stream_ptr(device)),

@@ -295,20 +295,7 @@ class NeuralODE(torch.nn.Module):
         _ffi.check(L.cfm_cnf_tc_euler_init(_ffi.ptr(st), _ffi.ptr(z), _ffi.ptr(P["x"]), _ffi.ptr(P["ll"]),
                                            _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), _ffi.ptr(traj), _ffi.ptr(t_span),
                                            n_span, seed, B, D, _ffi.stream_ptr(dev)), "cfm_cnf_tc_euler_init")
-        first = 0
-        if not self.use_cuda_graph or P["graph"] is None:
-            step()  # (the first call of a plan loads every kernel before the capture)
-            first = 1
-            if self.use_cuda_graph and n_span > 2:
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    step()
-                P["graph"] = g
-        for _ in range(first, n_span - 1):
-            if self.use_cuda_graph:
-                P["graph"].replay()
-            else:
-                step()
+        _ffi.replay_steps(P, step, n_span - 1, self.use_cuda_graph)
         self.stats = {"nfe": n_span - 1, "accepted": n_span - 1, "rejected": 0,
                       "graph": self.use_cuda_graph and P["graph"] is not None}
         return traj
@@ -339,12 +326,7 @@ class NeuralODE(torch.nn.Module):
         dev = x0.device
         B, D = x0.shape  # D: state columns
         n_span = t_span.numel()
-        ps = []
-        for lin in mlp._linears():
-            for p in (lin.weight, lin.bias):
-                if p.device != dev or p.dtype != torch.float32:
-                    raise _ffi.CfmLibraryError("MLP parameters must be fp32 on the input's CUDA device")
-                ps.append(p.detach().contiguous())
+        ps = mlp._device_params(dev)
         traj = torch.empty((n_span, B, D), dtype=torch.float32, device=dev)
         st = torch.zeros(ctypes_sizeof_state(), dtype=torch.uint8, device=dev)
         dim = mlp.dim if cnf else D

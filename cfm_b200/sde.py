@@ -126,16 +126,6 @@ def _tables_for(ts, dt, dev):
     return hit
 
 
-def _weights(mlp, dev):
-    ps = []
-    for lin in mlp._linears():
-        for p in (lin.weight, lin.bias):
-            if p.device != dev or p.dtype != torch.float32:
-                raise _ffi.CfmLibraryError("SDE net parameters must be fp32 on the input's CUDA device")
-            ps.append(p.detach().contiguous())
-    return ps
-
-
 @torch.no_grad()
 def sdeint(sde, y0, ts, bm=None, method=None, dt=1e-3, adaptive=False, logqp=False, **unsupported):
     """Subset of torchsde.sdeint: fixed-step Euler-Maruyama of a ``cfm_b200.SDE`` with two
@@ -173,7 +163,7 @@ def sdeint(sde, y0, ts, bm=None, method=None, dt=1e-3, adaptive=False, logqp=Fal
             "shared memory (one kernel), or in the tensor-core class: B >= 128, dim >= 32, dim and w multiples of 8, "
             "w >= 32")
     dev = y0.device
-    pd, psc = (_weights(drift, dev), _weights(score, dev)) if small else (None, None)
+    pd, psc = (drift._device_params(dev), score._device_params(dev)) if small else (None, None)
     with torch.cuda.device(dev):
         tables = _tables_for(ts_host, dt, dev)
         grid, out_begin, out_a, out_b, grid_host = tables
@@ -262,17 +252,4 @@ def _tc_euler(sde, drift, score, x0, tables, seed, inc, ys):
     _ffi.check(L.cfm_sde_tc_init(
         _ffi.ptr(P["st"]), _ffi.ptr(x0), _ffi.ptr(P["y"]), _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), _ffi.ptr(ys),
         _ffi.ptr(inc), seed, _ffi.ptr(tables[0]), n_steps, B, D, _ffi.stream_ptr(dev)), "cfm_sde_tc_init")
-    first = 0
-    if _EAGER or P["graph"] is None:
-        _tc_enqueue_step(sde, drift, P, B, D, dev)
-        first = 1
-        if not _EAGER and n_steps > 1:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                _tc_enqueue_step(sde, drift, P, B, D, dev)
-            P["graph"] = g
-    for _ in range(first, n_steps):
-        if _EAGER:
-            _tc_enqueue_step(sde, drift, P, B, D, dev)
-        else:
-            P["graph"].replay()
+    _ffi.replay_steps(P, lambda: _tc_enqueue_step(sde, drift, P, B, D, dev), n_steps, not _EAGER)
