@@ -9,14 +9,19 @@
   (``stats["nfe"]``).  J eps is a forward-mode tangent (``torch.func.jvp``); the reference writes the same number as
   ``(vjp(eps)[0] * eps).sum()`` per row (tests/test_cnf_tc_host.py checks the two agree).
 * ``magnitudes``: per-row float64 magnitude chains of one evaluation, the scales the error bounds of
-  tests/test_gpu_cnf_tc.py are stated in.
+  tests/test_gpu_cnf_tc.py are stated in; ``EPS_GEMM``, ``DIV_K`` and ``F_K``: those bounds (derived there), shared
+  by every test of the tensor-core samplers; ``lipschitz``: the growth rate the trajectory bounds carry.
 """
+import math
+
 import numpy as np
 import torch
 
 from oracle import sde as osde
 
 _MASK = np.uint64(0xFFFFFFFF)
+EPS_GEMM = 1e-6
+DIV_K, F_K = 10 * EPS_GEMM, 16 * EPS_GEMM
 
 
 def device_rademacher(seed, n, rows, cols):
@@ -120,3 +125,10 @@ def magnitudes(state, t, x, eps, act, eps_gemm):
     F = a.abs() @ W[3].abs().T + b[3].abs()
     S = (eps.abs() * (u @ W[3].abs().T)).sum(1)
     return F, S
+
+
+def lipschitz(mc, act):
+    """A Lipschitz bound of the MLP ``mc`` in x: the product of its layers' spectral norms times max|act'|^3."""
+    slope = 1.0507009873554805 * 1.6732632423543772 if act == "selu" else 1.1
+    norms = [torch.linalg.matrix_norm(mc.net[li].weight.double(), ord=2).item() for li in (0, 2, 4, 6)]
+    return math.prod(norms) * slope ** 3

@@ -21,6 +21,7 @@ import torch
 
 import cnf_oracle as co
 import cnf_tc_oracle as ho
+import tc_sampler_cases as tc
 from oracle import vector_field as vf
 
 import cfm_b200
@@ -28,8 +29,7 @@ from cfm_b200 import _ffi
 
 DEV = "cuda:0"
 pytestmark = pytest.mark.gpu
-EPS_GEMM = 1e-6
-DIV_K, F_K = 10 * EPS_GEMM, 16 * EPS_GEMM
+EPS_GEMM, DIV_K, F_K = ho.EPS_GEMM, ho.DIV_K, ho.F_K
 ESTS = ("hutch_gaussian", "hutch_rademacher")
 EST_CODE = {"hutch_gaussian": _ffi.HUTCH_GAUSSIAN, "hutch_rademacher": _ffi.HUTCH_RADEMACHER}
 
@@ -54,40 +54,40 @@ def _state(mc):
     return {k: v.detach() for k, v in mc.state_dict().items()}
 
 
-def _field(m, x, t, est, seed, n):
-    """One device evaluation through the C entry (fp32 x, split inside); the ordinal is passed as *ord + 2."""
+def _field(m, x, t, est, seed, n, pair=None, f=None, div=None, ws=None):
+    """One device evaluation through the C entry (fp32 x, split inside, or the operand pair ``pair`` = (hi, lo) with
+    x None); the ordinal is passed as *ord + 2.  ``f``, ``div`` and ``ws`` default to fresh buffers of x's batch."""
     L = _ffi.lib()
-    B, D = x.shape
-    blob = m._prepared(True, x.device)
-    ws = _ffi.workspace(L.cfm_cnf_tc_workspace_bytes(B, D, m.w), DEV)
-    f = torch.empty(B, D, device=DEV)
-    div = torch.empty(B, device=DEV)
+    B, D = x.shape if x is not None else pair[0].shape
+    blob = m._prepared(True, torch.device(DEV))
+    ws = _ffi.workspace(L.cfm_cnf_tc_workspace_bytes(B, D, m.w), DEV) if ws is None else ws
+    f = torch.empty(B, D, device=DEV) if f is None else f
+    div = torch.empty(B, device=DEV) if div is None else div
     tt = torch.tensor([t], dtype=torch.float32, device=DEV)
     sd = torch.tensor([seed], dtype=torch.int64, device=DEV)
     nn = torch.tensor([n - 2], dtype=torch.int32, device=DEV)
+    hi, lo = pair if pair is not None else (None, None)
     _ffi.check(L.cfm_cnf_tc_field_f32(
-        _ffi.ptr(blob), _ffi.ptr(x), None, None, B, D, m.w, m.act, EST_CODE[est], _ffi.ptr(tt), _ffi.ptr(sd),
-        _ffi.ptr(nn), 2, _ffi.ptr(f), _ffi.ptr(div), _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(DEV)),
+        _ffi.ptr(blob), _ffi.ptr(x), _ffi.ptr(hi), _ffi.ptr(lo), B, D, m.w, m.act, EST_CODE[est], _ffi.ptr(tt),
+        _ffi.ptr(sd), _ffi.ptr(nn), 2, _ffi.ptr(f), _ffi.ptr(div), _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(DEV)),
         "cfm_cnf_tc_field_f32")
     return f, div
 
 
-def _lip(mc, act):
-    slope = 1.0507009873554805 * 1.6732632423543772 if act == "selu" else 1.1
-    norms = [torch.linalg.matrix_norm(mc.net[li].weight.double(), ord=2).item() for li in (0, 2, 4, 6)]
-    return math.prod(norms) * slope ** 3
-
-
 # ---- one evaluation ---------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("act", ["selu", "silu"])
-@pytest.mark.parametrize("B,dim,w", [(256, 784, 256), (300, 64, 128), (129, 32, 32)])
-def test_one_evaluation_every_row_against_float64(B, dim, w, act):
-    m, mc = _pair(dim, w, dim + w, act)
-    x = torch.randn(B, dim, generator=torch.Generator().manual_seed(B)).to(DEV)
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def every_row_against_float64(m, mc, x, act, label):
+    """Both estimators at one (t, x): div within DIV_K S and f within F_K F of the float64 field on every row; f
+    bit-identical to the per-layer forward where m.vector_field takes it (w != 256 or dim < 64), within F_K F of the
+    fused forward elsewhere.  Prints the worst ratio to each gate."""
+    B, dim = x.shape
     t = 0.3
     with torch.no_grad():
         y = m.vector_field(t, x)
-    per_layer = not (w == 256 and dim >= 64)
+    per_layer = not (m.w == 256 and dim >= 64)
     for k, est in enumerate(ESTS):
         seed, n = 1234 + k, 9
         f, div = _field(m, x, t, est, seed, n)
@@ -97,10 +97,24 @@ def test_one_evaluation_every_row_against_float64(B, dim, w, act):
         err = (div.double() - ref).abs()
         assert bool((err <= DIV_K * S).all()), (est, float((err / S).max()))
         assert bool(((f.double() - ref_f).abs() <= F_K * F).all()), (est, float(((f.double() - ref_f).abs() / F).max()))
+        print(f"margins field {label} {act} {est}: div {float((err / (DIV_K * S)).max()):.2e} "
+              f"f {float(((f.double() - ref_f).abs() / (F_K * F)).max()):.3f} of the gate")
         if per_layer:  # the primal epilogue is the per-layer forward's: the same bits
             assert torch.equal(f, y)
-        else:
+        else:  # the fused forward
             assert float((f - y).abs().max()) <= 1e-5 * float(y.abs().max())
+            assert bool(((f.double() - y.double()).abs() <= F_K * F).all())
+
+
+@pytest.mark.parametrize("act", ["selu", "silu"])
+@pytest.mark.parametrize("B,dim,w", [(256, 784, 256), (300, 64, 128), (129, 32, 32)] + tc.FIELD_SHAPES)
+def test_one_evaluation_every_row_against_float64(B, dim, w, act):
+    """Also at the edges of tests/tc_sampler_cases.py: partial hidden and output chunks, 8-column N tiles, K tails,
+    more tiles than CTAs in every GEMM, one-row last M tiles, 1 to 25 fold chunks."""
+    B = tc.batch(B, _sms())
+    m, mc = _pair(dim, w, dim + w, act)
+    x = torch.randn(B, dim, generator=torch.Generator().manual_seed(B)).to(DEV)
+    every_row_against_float64(m, mc, x, act, f"{B}x{dim}x{w}")
 
 
 @pytest.mark.parametrize("est", ESTS)
@@ -152,21 +166,27 @@ def _seed_of(seed=77):
     return int(torch.randint(0, 2**63 - 1, (), dtype=torch.int64))
 
 
-@pytest.mark.parametrize("direction", ["forward", "reverse"])
+# (direction, shape): the first shape keeps the test's original ids
+_EULER = [pytest.param(d, s, id=d if s == tc.EULER_SHAPES[0] else f"{d}-{s[0]}x{s[1]}x{s[2]}")
+          for s in tc.EULER_SHAPES for d in ("forward", "reverse")]
+
+
+@pytest.mark.parametrize("direction,shape", _EULER)
 @pytest.mark.parametrize("est", ESTS)
-def test_euler_trajectory_against_float64_and_plain_wide_euler(est, direction):
-    B, dim, w, act = 256, 64, 128, "selu"
+def test_euler_trajectory_against_float64_and_plain_wide_euler(est, direction, shape):
+    B, dim, w, steps = shape
+    act = "selu"
     m, mc = _pair(dim, w, 11, act, scale=0.5)
-    lip = _lip(mc, act)
+    lip = ho.lipschitz(mc, act)
     assert lip < 2
     z = torch.cat([torch.randn(B, dim, generator=torch.Generator().manual_seed(12)), torch.zeros(B, 1)], 1).to(DEV)
-    span = torch.linspace(0, 1, 21) if direction == "forward" else torch.linspace(1, 0, 21)
+    span = torch.linspace(0, 1, steps + 1) if direction == "forward" else torch.linspace(1, 0, steps + 1)
     node = cfm_b200.NeuralODE(cfm_b200.cnf_wrapper(m, likelihood_estimator=est), solver="euler")
     traj = _seeded(node, z, span)
-    assert traj.shape == (21, B, dim + 1) and node.stats["nfe"] == 20 and node.stats["graph"]
+    assert traj.shape == (steps + 1, B, dim + 1) and node.stats["nfe"] == steps and node.stats["graph"]
     field = _Tracked(mc, est, _seed_of(), B, dim, act)
     ref = co.euler_any_direction(field, z.double(), span.double().to(DEV))
-    assert field.probes.n == 20
+    assert field.probes.n == steps
     h = (span[1:] - span[:-1]).abs().double().tolist()
     grow = math.exp(lip)
     bx = torch.zeros(B, dim, dtype=torch.float64, device=DEV)
@@ -178,18 +198,31 @@ def test_euler_trajectory_against_float64_and_plain_wide_euler(est, direction):
     err = (traj.double() - ref).abs()
     assert bool((err[-1, :, :dim] <= bx).all()), float((err[-1, :, :dim] / bx).max())
     assert bool((err[-1, :, dim] <= bl).all()), float((err[-1, :, dim] / bl).max())
-    # the x columns are those of the plain wide Euler trajectory on this per-layer shape, bit for bit
+    print(f"margins euler {B}x{dim}x{w} {est} {direction}: x {float((err[-1, :, :dim] / bx).max()):.3f} "
+          f"ll {float((err[-1, :, dim] / bl).max()):.2e} of the gate")
+    # eager enqueue gives the bits of the graph replay
+    node.use_cuda_graph = False
+    assert torch.equal(_seeded(node, z, span), traj)
+    if w == 256 and dim >= 64:  # the plain wide Euler takes the fused forward there
+        return
+    # the x columns are those of the plain wide Euler trajectory on a per-layer shape, bit for bit
     plain = cfm_b200.NeuralODE(cfm_b200.torch_wrapper(m), solver="euler")
     with torch.no_grad():
         px = plain.trajectory(z[:, :dim].contiguous(), span)
     assert torch.equal(traj[..., :dim], px)
 
 
-@pytest.mark.parametrize("direction", ["forward", "reverse"])
-def test_dopri5_takes_the_oracle_step_sequence(direction):
-    B, dim, w, act, est = 256, 64, 128, "silu", "hutch_gaussian"
+# (direction, B): B (D + 1) = 1, 2, 3 mod 4 puts the stage outputs f = k[i] at every 4-byte offset mod 16; the first
+# batch keeps the test's original ids
+_DOPRI5 = [pytest.param(d, B, id=d if B == tc.DOPRI5_BATCHES[0] else f"{d}-B{B}")
+           for B in tc.DOPRI5_BATCHES for d in ("forward", "reverse")]
+
+
+@pytest.mark.parametrize("direction,B", _DOPRI5)
+def test_dopri5_takes_the_oracle_step_sequence(direction, B):
+    (dim, w), act, est = tc.DOPRI5_SHAPE, "silu", "hutch_gaussian"
     m, mc = _pair(dim, w, 21, act, scale=0.5)
-    lip = _lip(mc, act)
+    lip = ho.lipschitz(mc, act)
     z = torch.cat([torch.randn(B, dim, generator=torch.Generator().manual_seed(22)), torch.zeros(B, 1)], 1).to(DEV)
     span = torch.linspace(0, 1, 3) if direction == "forward" else torch.linspace(1, 0, 3)
     node = cfm_b200.NeuralODE(cfm_b200.cnf_wrapper(m, likelihood_estimator=est), solver="dopri5", atol=1e-5,
@@ -208,6 +241,8 @@ def test_dopri5_takes_the_oracle_step_sequence(direction):
     err = (traj.double() - ref).abs()
     assert bool((err[..., :dim] <= bx).all()), float((err[..., :dim] / bx).max())
     assert bool((err[..., dim] <= bl).all()), float((err[..., dim] / bl).max())
+    print(f"margins dopri5 B={B} {direction}: x {float((err[..., :dim] / bx).max()):.3f} "
+          f"ll {float((err[..., dim] / bl).max()):.2e} of the gate")
     assert torch.equal(_seeded(node, z, span), traj)  # the captured step and init replay the same bits
     node.use_cuda_graph = False
     node._plans.clear()

@@ -5,10 +5,12 @@ restatement of torchsde's fixed-step Euler (oracle/sde.py).
 CPU: argument checks before any CUDA call, the class predicate against the tensor-core shape rule, and the kernel
 instantiations in the built library.
 GPU: parity with supplied increments (per-layer path, the C3 model, a ragged K chunk, CTAs that switch from drift to
-score slabs); the pair launch against two single launches, bit for bit; bit identity with the wide Euler ODE path;
-one noise stream across both classes; rows independent of the batch; graph against eager replay and the launch count;
-weights updated in place; dispatch and refusals."""
+score slabs), by max-abs and per entry; the pair launch against two single launches, bit for bit, also across the slab
+schedules of tests/tc_sampler_cases.py; bit identity with the wide Euler ODE path; one noise stream across both
+classes; the device's own noise on a non-uniform step grid against float64, per entry; rows independent of the batch;
+graph against eager replay and the launch count; weights updated in place; dispatch and refusals."""
 import ctypes
+import math
 import re
 import subprocess
 
@@ -16,6 +18,8 @@ import numpy as np
 import pytest
 import torch
 
+import cnf_tc_oracle as ho
+import tc_sampler_cases as tc
 from oracle import sde as osde
 from oracle import vector_field as vf
 
@@ -100,6 +104,45 @@ def _radius_uniform(seed, n, rows, cols):
     return np.where((c & np.uint64(2)).astype(bool), u[..., 2], u[..., 0])
 
 
+class _Bounded:
+    """The float64 drift + score that osde.euler_sdeint calls once per step, carrying the per-entry error bound of the
+    device trajectory along.  Step n adds
+      * h_n 16 EPS_GEMM (F_d + F_s): both nets' fp16x3 forwards, F = cnf_tc_oracle.magnitudes on the oracle's state;
+      * 4 units of 2^-24 of |y_n| + h_n |f_n| + sigma |dW_n|: the fp32 roundings of d + s, the fma, sigma dW and the sum;
+      * sigma inc_err[n]: the error of the device's own increment (zero when the increments are supplied).
+    Output k gets the sum up to the step that brackets it times exp(T Lip), plus 4 units of 2^-24 of the magnitudes of
+    the two states it interpolates (the fp32 interpolation and its fp32 weights)."""
+
+    def __init__(self, nets, act, ts, dt, sigma, incs, inc_err=None):
+        self.nets, self.act, self.sigma, self.incs, self.inc_err = nets, act, sigma, incs, inc_err
+        self.states = [{k: v.detach() for k, v in m.state_dict().items()} for m in nets]
+        self.grid, bracket = osde.step_grid(ts, dt)
+        self.outputs = {}  # step n -> the outputs k it brackets
+        for k, n in enumerate(bracket, 1):
+            self.outputs.setdefault(n, []).append(k)
+        self.n, self.cum, self.at = 0, 0.0, {}
+
+    def __call__(self, t, y):
+        n = self.n
+        tt = torch.tensor(t, dtype=torch.float64, device=y.device)
+        f = sum(vf.wrapped_forward(m, tt, y) for m in self.nets)
+        F = sum(ho.magnitudes(st, t, y, torch.zeros_like(y), self.act, ho.EPS_GEMM)[0] for st in self.states)
+        h = float(self.grid[n + 1] - self.grid[n])
+        mag = y.abs() + h * f.abs() + self.sigma * self.incs[n].abs()
+        self.cum = self.cum + h * ho.F_K * F + 4 * 2.0**-24 * mag
+        if self.inc_err is not None:
+            self.cum = self.cum + self.sigma * self.inc_err[n]
+        for k in self.outputs.get(n, []):
+            self.at[k] = (self.cum, mag + y.abs())
+        self.n += 1
+        return f
+
+    def bound(self, grow):
+        first = torch.zeros_like(self.at[1][1])  # ys[0] is y0 itself
+        return torch.stack([first] + [grow * self.at[k][0] + 4 * 2.0**-24 * self.at[k][1]
+                                      for k in range(1, len(self.at) + 1)])
+
+
 def _split(x):
     """The fp16x3 operand pair of x (finite, within fp16 range): hi = fp16(x), lo = fp16((x - hi) 2^11)."""
     hi = x.half()
@@ -179,28 +222,39 @@ _SHAPES = [(200, 32, 128, "selu"), (1000, 784, 256, "selu"), (300, 200, 256, "si
 @pytest.mark.parametrize("kind", ["offgrid", "sf2m"])
 @pytest.mark.parametrize("B,dim,w,act", _SHAPES)
 def test_parity_with_supplied_increments(B, dim, w, act, kind, record_property):
+    """Two gates: the trajectory's max-abs, and per entry the bound _Bounded carries step by step."""
     B = B or _many_slabs_batch()
-    sde, f64 = _sde(dim, w, seed=dim + w, act=act, sigma=0.8)
+    (d, dc), (s, sc) = _nets(dim, w, seed=dim + w, act=act)
+    sde = cfm_b200.SDE(d, s, input_size=(dim,), sigma=0.8)
     ts, dt = _TS[kind]
     y0 = torch.randn(B, dim, generator=torch.Generator().manual_seed(dim)).to(DEV)
     bm = DeviceBM(B, dim, seed=w + dim)
     ys = cfm_b200.sdeint(sde, y0, ts, bm=bm, method="euler", dt=dt)
     assert ys.shape == (len(ts), B, dim) and ys.dtype == torch.float32 and ys.device.type == "cuda"
     assert torch.equal(ys[0], y0)
-    ref = osde.euler_sdeint(f64, 0.8, y0.double(), ts, dt, torch.stack(bm.incs))
+    incs = torch.stack(bm.incs).double()
     del bm
-    err = (ys.double() - ref).abs().max().item()
+    field = _Bounded((dc, sc), act, ts, dt, 0.8, incs)
+    ref = osde.euler_sdeint(field, 0.8, y0.double(), ts, dt, incs)
+    err = (ys.double() - ref).abs()
     gate = 1e-4 * max(1.0, ref.abs().max().item())
-    record_property("err_over_gate", err / gate)
-    assert err <= gate, (err, gate)
+    record_property("err_over_gate", err.max().item() / gate)
+    assert err.max().item() <= gate, (err.max().item(), gate)
+    lip = ho.lipschitz(dc, act) + ho.lipschitz(sc, act)
+    bound = field.bound(math.exp(float(ts[-1] - ts[0]) * lip))
+    print(f"margins sde parity {B}x{dim}x{w} {kind}: max-abs {err.max().item() / gate:.3f}, per entry "
+          f"{float((err / bound)[1:].max()):.2e} of the gate (Lip {lip:.1f})")
+    assert bool((err <= bound).all()), float((err / bound)[1:].max())
 
 
 # ---- GPU: the pair launch is two single launches -------------------------------------------------------------------
 @gpu
 @pytest.mark.parametrize("act", ["selu", "silu"])
-@pytest.mark.parametrize("B,dim,w", [(s[0], s[1], s[2]) for s in _SHAPES])
+@pytest.mark.parametrize("B,dim,w", [(s[0], s[1], s[2]) for s in _SHAPES] + tc.PAIR_SHAPES)
 def test_pair_launch_equals_two_single_launches_bit_for_bit(B, dim, w, act):
-    B = B or _many_slabs_batch()
+    """Also at the slab schedules of tests/tc_sampler_cases.py: one slab per net, one slab per CTA, 2 S = grid + 2,
+    S >= SMs (two drift slabs before a score slab) and a ragged drift slab followed by a score slab on one CTA."""
+    B = _many_slabs_batch() if B is None else tc.batch(B, _sms())
     (d, _), (s, _) = _nets(dim, w, seed=3 * dim + w, act=act)
     L = _ffi.lib()
     x = torch.randn(B, dim, generator=torch.Generator().manual_seed(5)).to(DEV)
@@ -268,6 +322,50 @@ def test_one_noise_stream_across_the_small_and_tensor_core_classes():
         assert near_one.mean() < 1e-3
         ok = np.abs(dz[n] - z) <= 1e-5 * np.maximum(1.0, np.abs(z))
         assert (ok | near_one).all(), n
+
+
+# ---- GPU: the device's own noise against float64 -------------------------------------------------------------------
+@gpu
+@pytest.mark.parametrize("B,dim,w,act", tc.NOISE_SHAPES)
+def test_own_noise_against_float64_entry_by_entry(B, dim, w, act):
+    """bm=None on a step grid whose h changes (an off-grid ts, a dt that does not divide the span): the step kernel
+    draws dW_n = sqrt(h_n) z_n itself.  On the rows of tc.noise_rows (the first, both sides of every 128-row slab
+    boundary, the last) the trajectory stays within _Bounded's per-entry bound of the float64 Euler loop driven by
+    osde.device_normals(seed, n) sqrt(h_n).  The device increment errs by at most sqrt(h_n) (2^-23 / rad + 2^-20 rad +
+    2^-23 |z|) per entry, rad = sqrt(-2 log u) the Box-Muller radius: the fp32 rounding of a radius uniform u >= 1/2
+    moves rad by up to 2^-24 / rad, logf, sqrtf, sincospif and the angle's rounding by a few units of 2^-24 of rad,
+    the products by 2^-24 each."""
+    (d, dc), (s, sc) = _nets(dim, w, seed=150 + dim, act=act)
+    with torch.no_grad():
+        for m in (d, dc, s, sc):
+            for li in (2, 4, 6):
+                m.net[li].weight.mul_(0.4)
+    lip = ho.lipschitz(dc, act) + ho.lipschitz(sc, act)
+    assert lip < 2, lip
+    sigma, dt = tc.NOISE_SIGMA, tc.NOISE_DT
+    sde = cfm_b200.SDE(d, s, input_size=(dim,), sigma=sigma)
+    ts = torch.tensor(tc.NOISE_TS, dtype=torch.float32)
+    y0 = torch.randn(B, dim, generator=torch.Generator().manual_seed(151)).to(DEV)
+    torch.manual_seed(152)
+    ys = cfm_b200.sdeint(sde, y0, ts, method="euler", dt=dt)
+    torch.manual_seed(152)
+    seed = int(torch.randint(0, 2**63 - 1, (), dtype=torch.int64))
+    rows = tc.noise_rows(B)
+    grid, _ = osde.step_grid(ts, dt)
+    incs, errs = [], []
+    for n in range(len(grid) - 1):
+        root = float(grid[n + 1] - grid[n]) ** 0.5
+        z = osde.device_normals(seed, n, rows, dim)
+        rad = np.sqrt(-2.0 * np.log(_radius_uniform(seed, n, rows, dim)))
+        incs.append(torch.from_numpy(z * root))
+        errs.append(torch.from_numpy(root * (2.0**-23 / rad + 2.0**-20 * rad + 2.0**-23 * np.abs(z))))
+    incs, errs = torch.stack(incs).to(DEV), torch.stack(errs).to(DEV)
+    field = _Bounded((dc, sc), act, ts, dt, sigma, incs, errs)
+    ref = osde.euler_sdeint(field, sigma, y0[rows].double(), ts, dt, incs)
+    bound = field.bound(math.exp(float(ts[-1] - ts[0]) * lip))
+    err = (ys[:, rows].double() - ref).abs()
+    print(f"margins sde own noise {B}x{dim}x{w} {act}: {float((err / bound)[1:].max()):.3f} of the gate")
+    assert bool((err <= bound).all()), float((err / bound)[1:].max())
 
 
 # ---- GPU: rows independent of the batch; seeding --------------------------------------------------------------------
