@@ -7,9 +7,10 @@ instantiations in the built library.
 GPU: parity with supplied increments (per-layer path, the C3 model, a ragged K chunk, CTAs that switch from drift to
 score slabs), by max-abs and per entry; the pair launch against two single launches, bit for bit, also across the slab
 schedules of tests/tc_sampler_cases.py; bit identity with the wide Euler ODE path; one noise stream across both
-classes; the device's own noise on a non-uniform step grid against float64, per entry; rows independent of the batch;
+classes; the device's own noise on a non-uniform step grid against float64, per entry (small_field_oracle.Bounded); rows independent of the batch;
 graph against eager replay and the launch count; weights updated in place; dispatch and refusals."""
 import ctypes
+import functools
 import math
 import re
 import subprocess
@@ -19,6 +20,7 @@ import pytest
 import torch
 
 import cnf_tc_oracle as ho
+import small_field_oracle as sfo
 import tc_sampler_cases as tc
 from oracle import sde as osde
 from oracle import vector_field as vf
@@ -93,54 +95,9 @@ def _launches(fn):
     return out, L.cfm_launch_count() - before
 
 
-def _radius_uniform(seed, n, rows, cols):
-    """The float64 uniform under the square root of osde.device_normals' Box-Muller, per (row, column)."""
-    rows = np.asarray(rows, dtype=np.uint64)[:, None]
-    c = np.arange(cols, dtype=np.uint64)[None, :]
-    ctr = np.stack(np.broadcast_arrays(c >> np.uint64(2), rows & np.uint64(0xFFFFFFFF), rows >> np.uint64(32),
-                                       np.full_like(c, n)), axis=-1)
-    x = osde.philox4x32_10(ctr, np.array([seed & 0xFFFFFFFF, seed >> 32], dtype=np.uint64))
-    u = (x >> np.uint32(8)).astype(np.float64) * 2.0**-24 + 2.0**-25
-    return np.where((c & np.uint64(2)).astype(bool), u[..., 2], u[..., 0])
-
-
-class _Bounded:
-    """The float64 drift + score that osde.euler_sdeint calls once per step, carrying the per-entry error bound of the
-    device trajectory along.  Step n adds
-      * h_n 16 EPS_GEMM (F_d + F_s): both nets' fp16x3 forwards, F = cnf_tc_oracle.magnitudes on the oracle's state;
-      * 4 units of 2^-24 of |y_n| + h_n |f_n| + sigma |dW_n|: the fp32 roundings of d + s, the fma, sigma dW and the sum;
-      * sigma inc_err[n]: the error of the device's own increment (zero when the increments are supplied).
-    Output k gets the sum up to the step that brackets it times exp(T Lip), plus 4 units of 2^-24 of the magnitudes of
-    the two states it interpolates (the fp32 interpolation and its fp32 weights)."""
-
-    def __init__(self, nets, act, ts, dt, sigma, incs, inc_err=None):
-        self.nets, self.act, self.sigma, self.incs, self.inc_err = nets, act, sigma, incs, inc_err
-        self.states = [{k: v.detach() for k, v in m.state_dict().items()} for m in nets]
-        self.grid, bracket = osde.step_grid(ts, dt)
-        self.outputs = {}  # step n -> the outputs k it brackets
-        for k, n in enumerate(bracket, 1):
-            self.outputs.setdefault(n, []).append(k)
-        self.n, self.cum, self.at = 0, 0.0, {}
-
-    def __call__(self, t, y):
-        n = self.n
-        tt = torch.tensor(t, dtype=torch.float64, device=y.device)
-        f = sum(vf.wrapped_forward(m, tt, y) for m in self.nets)
-        F = sum(ho.magnitudes(st, t, y, torch.zeros_like(y), self.act, ho.EPS_GEMM)[0] for st in self.states)
-        h = float(self.grid[n + 1] - self.grid[n])
-        mag = y.abs() + h * f.abs() + self.sigma * self.incs[n].abs()
-        self.cum = self.cum + h * ho.F_K * F + 4 * 2.0**-24 * mag
-        if self.inc_err is not None:
-            self.cum = self.cum + self.sigma * self.inc_err[n]
-        for k in self.outputs.get(n, []):
-            self.at[k] = (self.cum, mag + y.abs())
-        self.n += 1
-        return f
-
-    def bound(self, grow):
-        first = torch.zeros_like(self.at[1][1])  # ys[0] is y0 itself
-        return torch.stack([first] + [grow * self.at[k][0] + 4 * 2.0**-24 * self.at[k][1]
-                                      for k in range(1, len(self.at) + 1)])
+# the step-by-step trajectory bound and the Box-Muller radius uniform, shared with the small SDE kernel's tests
+_radius_uniform = sfo.radius_uniform
+_Bounded = functools.partial(sfo.Bounded, net_err=sfo.tc_net_err)
 
 
 def _split(x):
