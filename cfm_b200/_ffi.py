@@ -45,6 +45,12 @@ class CnfTcState(C.Structure):
                 ("n_steps", C.c_int32), ("t", C.c_float), ("ticket", C.c_uint32)]
 
 
+class GradTcState(C.Structure):
+    """Mirror of ``cfm_grad_tc_state`` (include/cfm_b200.h)."""
+    _fields_ = [("traj", C.c_void_p), ("t_span", C.c_void_p), ("n", C.c_int32), ("n_steps", C.c_int32),
+                ("t", C.c_float), ("ticket", C.c_uint32)]
+
+
 _p, _i, _i64, _f, _d, _sz =C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double, C.c_size_t
 
 # name -> (restype, argtypes); must list every symbol include/cfm_b200.h declares
@@ -107,6 +113,13 @@ SIGNATURES = {
     "cfm_cnf_tc_field_f32": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _p, _sz, _p]),
     "cfm_cnf_tc_euler_init": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i, C.c_uint64, _i, _i, _p]),
     "cfm_cnf_tc_euler_step": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _i, _p]),
+    "cfm_grad_tc_supported": (_i, [_i, _i, _i]),
+    "cfm_grad_tc_prepared_bytes": (_sz, [_i, _i]),
+    "cfm_grad_tc_prepare": (_i, [_p, _i, _i, _p, _sz, _p]),
+    "cfm_grad_tc_workspace_bytes": (_sz, [_i, _i, _i]),
+    "cfm_grad_tc_field_f32": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _sz, _p]),
+    "cfm_grad_tc_euler_init": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p]),
+    "cfm_grad_tc_euler_step": (_i, [_p, _p, _p, _p, _p, _i, _i, _p]),
     "cfm_mlp_small_train_supported":(_i, [_i64, _i, _i, _i]),
     "cfm_mlp_small_train_workspace_bytes": (_sz, [_i64, _i, _i, _i]),
     "cfm_mlp_small_mse_grad_f32": (_i, [_p] * 8 + [_i, _i, _i, _i, _p, _p, _p, _p, _i64, _i, _p, _p, _p, _sz, _p]),

@@ -15,7 +15,8 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcfm_b200.so")
 SOURCES = ["api.cu", "sqdist.cu", "sqdist_h3.cu", "sinkhorn.cu", "sinkhorn_v2.cu", "sample.cu", "assign.cu",
            "gather.cu", "flow.cu", "mlp.cu", "mlp_h3.cu", "rk.cu", "ode_small.cu", "train_small.cu",
-           "action_train.cu", "cnf_train.cu", "train_tc.cu", "sde_tc.cu", "cnf_tc.cu"]
+           "action_train.cu", "cnf_train.cu", "train_tc.cu", "sde_tc.cu", "cnf_tc.cu",
+           "grad_tc.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-O3,-Wall", "--expt-relaxed-constexpr", "-Xptxas", "-v"]

@@ -274,6 +274,19 @@ cnf_euler_step_kernel(cfm_cnf_tc_state* st, float4* __restrict__ x, float* __res
 
 }  // namespace
 
+// One hidden primal layer on its own: the split of act(pre) to (out_hi, out_lo) and act'(pre) to dact, all [B][w].
+// The gradient field of grad_tc.cu runs its layers 0 and 1 through this, on the same kernel instantiation.
+int cnf_tc_primal_hidden(const __half* ah, const __half* al, int batch, int K, const void* wh, const void* wl,
+                         int64_t ldw, int w, const float* bias, const float* inv_ws, const float* tcol,
+                         const float* t_dev, int act, float* dact, __half* out_hi, __half* out_lo, cudaStream_t s) {
+  CnfPrimalEpi pe;
+  pe.bias = bias; pe.inv_ws = inv_ws; pe.tcol = tcol; pe.t_dev = t_dev; pe.act = act; pe.dact = dact;
+  pe.out_hi = out_hi; pe.out_lo = out_lo; pe.f = nullptr; pe.ldo = w; pe.t = 0.f;
+  return launch_gemm_h3<CnfPrimalEpi, cnf_gemm_kernel<CnfPrimalEpi>>(ah, al, batch, K, reinterpret_cast<const __half*>(wh),
+                                                                     reinterpret_cast<const __half*>(wl), w, ldw, K, pe,
+                                                                     s);
+}
+
 }  // namespace cfm
 
 using namespace cfm;

@@ -75,6 +75,25 @@ class MLP(torch.nn.Module):
         self._blobs[key] = (ver, blob)
         return blob
 
+    def _grad_prepared(self, device):
+        """(forward blob, gradient blob) of a scalar action for the tensor-core gradient field (csrc/grad_tc.cu): the
+        gradient blob holds the transposed weight pairs of the reverse pass, built from the forward blob once per
+        weight version."""
+        fwd = self._prepared(True, device)
+        key = ("grad", device)
+        ver = (self._weights_key(), fwd.data_ptr())
+        hit = self._blobs.get(key)
+        if hit is not None and hit[0] == ver:
+            return fwd, hit[1]
+        L = _ffi.lib()
+        nbytes = L.cfm_grad_tc_prepared_bytes(self.dim, self.w)
+        blob = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            _ffi.check(L.cfm_grad_tc_prepare(_ffi.ptr(fwd), self.dim, self.w, _ffi.ptr(blob), nbytes,
+                                             _ffi.stream_ptr(device)), "cfm_grad_tc_prepare")
+        self._blobs[key] = (ver, blob)
+        return fwd, blob
+
     def _time_reversed(self):
         """The field f_(s, x) = -f(-s, x) as an MLP: W3, b3 and the time column of W0 negated.  A decreasing
         ``t_span`` is integrated as this field over ``-t_span`` (torchdyn's reparametrisation); negation is exact
@@ -184,7 +203,9 @@ class GradModel(torch.nn.Module):
     ``forward`` is plain PyTorch with ``create_graph=True``, so the action-matching loss backpropagates through it on
     any device; it needs autograd and fails under ``torch.no_grad()`` as the reference does.  Sampling
     ``torch_wrapper(GradModel(MLP(dim, out_dim=1, time_varying=True)))`` with ``cfm_b200.NeuralODE`` runs the forward
-    and reverse pass of the action in one kernel instead (csrc/ode_small.cu, gradient variant), and
+    and reverse pass of the action in one kernel instead (csrc/ode_small.cu, gradient variant) for w in {32, 64} and
+    dim <= 8, and on the tensor cores (csrc/grad_tc.cu: six GEMM launches per evaluation) for actions in the
+    tensor-core class (B >= 128, dim >= 32, dim and w multiples of 8, w >= 32; e.g. the MNIST shape), and
     ``cfm_b200.action_matching_loss(action, xt, t, x0, x1)`` computes the notebook's training loss and all parameter
     gradients of such an action in one kernel (csrc/action_train.cu) without this double backward."""
 

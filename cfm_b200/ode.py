@@ -21,8 +21,10 @@ state carries the log-density column, and the whole trajectory, trace included, 
 is accepted for models in the tensor-core class (B >= 128, dim >= 32, dim and w multiples of 8, w >= 32,
 out_dim == dim; e.g. the MNIST model): Hutchinson's eps . (J eps) with one device-drawn probe per evaluation
 (csrc/cnf_tc.cu), Euler with a captured step or dopri5 on the flat [x, ll] state.  So is
-``torch_wrapper(GradModel(MLP(time_varying=True, out_dim=1)))``, the
-action-matching field grad_x s(t, x) (gradient variant).
+``torch_wrapper(GradModel(MLP(time_varying=True, out_dim=1)))``, the action-matching field grad_x s(t, x): small
+actions (w in {32, 64}, dim <= 8) in the gradient variant of the one-launch kernel, actions in the tensor-core class
+(B >= 128, dim >= 32, dim and w multiples of 8, w >= 32; e.g. the MNIST shape) as a forward and a reverse pass of
+fp16x3 GEMMs (csrc/grad_tc.cu), Euler with a captured step or dopri5.
 
 A decreasing ``t_span`` is integrated as torchdyn does: dopri5 runs the field f_(s, x) = -f(-s, x) over
 s = -t_span (for the MLP only a different weight set, ``MLP._time_reversed``), because the step controller
@@ -140,6 +142,7 @@ class NeuralODE(torch.nn.Module):
         self.lockstep = None
         self._plans = {}
         self._cnf_plans = {}  # Hutchinson Euler: plan key -> buffers and the captured step graph
+        self._grad_plans = {}  # tensor-core gradient-field Euler, likewise
 
     def forward(self, x, t_span):
         traj = self.trajectory(x, t_span)
@@ -302,7 +305,9 @@ class NeuralODE(torch.nn.Module):
 
     def _grad_trajectory_on(self, mlp, x, t_span, dev):
         """torch_wrapper(GradModel(mlp)): the field grad_x mlp(t, x) through the gradient variant of the one-launch
-        kernel."""
+        kernel (w in {32, 64}, dim <= 8) or, for actions in the tensor-core class, through the forward and reverse GEMMs
+        of csrc/grad_tc.cu.  The two classes are disjoint (dim <= 8 against dim >= 32); any other shape raises before
+        any launch."""
         if self.lockstep is not None:
             raise NotImplementedError("GradModel: lock-step sharding is not supported; the gradient-field path "
                                       "integrates the whole batch in one single-device kernel")
@@ -310,11 +315,60 @@ class NeuralODE(torch.nn.Module):
             raise ValueError(f"GradModel: expected a state of shape (B, {mlp.dim}), got {tuple(x.shape)}")
         if t_span.numel() < 2:
             raise ValueError("GradModel: t_span needs at least two points")
-        if not _ffi.lib().cfm_ode_small_grad_supported(x.shape[0], mlp.dim, mlp.w):
+        L = _ffi.lib()
+        B = x.shape[0]
+        x0 = x.detach().float().contiguous()
+        if L.cfm_ode_small_grad_supported(B, mlp.dim, mlp.w):
+            return self._fused_small(mlp, x0, t_span.to(dev).contiguous(), grad=True)
+        if not (B < 2**31 and mlp.act in (_ffi.ACT_SELU, _ffi.ACT_SILU) and L.cfm_grad_tc_supported(B, mlp.dim, mlp.w)):
             raise NotImplementedError(
-                f"GradModel: no gradient-field kernel for B={x.shape[0]}, dim={mlp.dim}, w={mlp.w} (it takes w in "
-                "{32, 64}, dim <= 8 and batches whose state fits in shared memory)")
-        return self._fused_small(mlp, x.detach().float().contiguous(), t_span.to(dev).contiguous(), grad=True)
+                f"GradModel: no gradient-field kernel for B={B}, dim={mlp.dim}, w={mlp.w}: the one-launch kernel takes "
+                "w in {32, 64}, dim <= 8 and batches whose state fits in shared memory; the tensor-core class takes "
+                "B >= 128, dim >= 32, dim and w multiples of 8, w >= 32")
+        if self.solver == "euler":
+            return self._grad_tc_euler(mlp, x0, t_span.to(dev).contiguous())
+        return self._dopri5(mlp, x0, t_span.detach().cpu().contiguous())
+
+    def _grad_tc_euler(self, mlp, x, t_span):
+        """Euler over ``t_span`` for an action in the tensor-core class (csrc/grad_tc.cu): init, then per step the six
+        launches of one gradient-field evaluation and the step kernel, captured once as a CUDA graph per plan and
+        replayed."""
+        L = _ffi.lib()
+        dev = x.device
+        B, D, n_span = x.shape[0], mlp.dim, t_span.numel()
+        blob, gblob = mlp._grad_prepared(dev)
+        key = (id(mlp), B, D, str(dev), mlp._weights_key(), blob.data_ptr(), gblob.data_ptr(), mlp.act,
+               torch.cuda.current_stream(dev).cuda_stream)
+        P = self._grad_plans.get(key)
+        if P is None:
+            self._grad_plans.clear()  # one live plan: a new shape / new weights retire the old graph
+            st = torch.zeros(C.sizeof(_ffi.GradTcState), dtype=torch.uint8, device=dev)
+            P = {"st": st, "x": torch.empty((B, D), dtype=torch.float32, device=dev),
+                 "v": torch.empty((B, D), dtype=torch.float32, device=dev),
+                 "hi": torch.empty((B, D), dtype=torch.float16, device=dev),
+                 "lo": torch.empty((B, D), dtype=torch.float16, device=dev),
+                 "ws": _ffi.workspace(L.cfm_grad_tc_workspace_bytes(B, D, mlp.w), dev), "graph": None}
+            self._grad_plans[key] = P
+        st, ws = P["st"], P["ws"]
+        t_at = C.c_void_p(st.data_ptr() + _ffi.GradTcState.t.offset)
+
+        def step():  # on the current stream, which is the capture stream inside torch.cuda.graph
+            sp = _ffi.stream_ptr(dev)
+            _ffi.check(L.cfm_grad_tc_field_f32(
+                _ffi.ptr(blob), _ffi.ptr(gblob), None, _ffi.ptr(P["hi"]), _ffi.ptr(P["lo"]), B, D, mlp.w, mlp.act,
+                t_at, _ffi.ptr(P["v"]), _ffi.ptr(ws), ws.numel(), sp), "cfm_grad_tc_field_f32")
+            _ffi.check(L.cfm_grad_tc_euler_step(_ffi.ptr(st), _ffi.ptr(P["x"]), _ffi.ptr(P["v"]), _ffi.ptr(P["hi"]),
+                                                _ffi.ptr(P["lo"]), B, D, sp), "cfm_grad_tc_euler_step")
+
+        traj = torch.empty((n_span, B, D), dtype=torch.float32, device=dev)
+        P["span"] = t_span  # read through the state by every step: kept alive with the plan
+        _ffi.check(L.cfm_grad_tc_euler_init(_ffi.ptr(st), _ffi.ptr(x), _ffi.ptr(P["x"]), _ffi.ptr(P["hi"]),
+                                            _ffi.ptr(P["lo"]), _ffi.ptr(traj), _ffi.ptr(t_span), n_span, B, D,
+                                            _ffi.stream_ptr(dev)), "cfm_grad_tc_euler_init")
+        _ffi.replay_steps(P, step, n_span - 1, self.use_cuda_graph)
+        self.stats = {"nfe": n_span - 1, "accepted": n_span - 1, "rejected": 0,
+                      "graph": self.use_cuda_graph and P["graph"] is not None}
+        return traj
 
     # ------------------------------------------------------------------------------------
     def _fused_small(self, mlp, x0, t_span, cnf=False, grad=False):
@@ -390,8 +444,9 @@ class NeuralODE(torch.nn.Module):
         """Persistent buffers (+ the captured step graph) for one problem shape and weight version.  ``cnf``: the
         Hutchinson estimator of a cnf_wrapper state, laid out flat as the x block [B][D] followed by the ll block [B]
         (numel = B (D + 1)); every cfm_rk_* kernel takes that layout unchanged."""
+        grad = cnf is None and _grad_model(self.vf) is not None  # the action's gradient field (csrc/grad_tc.cu)
         key = (id(mlp), B, D, n_span, str(dev), mlp._weights_key(), mlp.mlp_algo, mlp.act, self.lockstep is not None,
-               cnf)
+               cnf, grad)
         P = self._plans.get(key)
         if P is not None:
             return P
@@ -416,11 +471,13 @@ class NeuralODE(torch.nn.Module):
         P["err_acc"] = st[off:off + 8].view(torch.float64)
         off = _ffi.RkState.done.offset  # int32: non-zero once t has reached t_end
         P["done_flag"] = st[off:off + 4].view(torch.int32)
-        if cnf is not None or mlp.tc_path(B):
+        if cnf is not None or grad or mlp.tc_path(B):
             # stage inputs go to the MLP as its fp16x3 tensor-core operand pair (hi, lo), written by the RK kernel
             P["xs_hi"] = torch.empty(shape, dtype=torch.float16, device=dev)
             P["xs_lo"] = torch.empty(shape, dtype=torch.float16, device=dev)
-        if cnf is None:
+        if grad:
+            self._grad_fields(mlp, P, B, D)
+        elif cnf is None:
             P["field"] = lambda t, x, out, n: mlp.vector_field(t, x, out=out)
             P["field_split"] = lambda t, hi, lo, out, skip, n: mlp.vector_field_split(t, hi, lo, out, skip_flag=skip)
         else:
@@ -446,6 +503,24 @@ class NeuralODE(torch.nn.Module):
                 _ffi.ptr(blob), _ffi.ptr(x), _ffi.ptr(hi), _ffi.ptr(lo), B, D, mlp.w, mlp.act, _HUTCH[est], _ffi.ptr(t),
                 _ffi.ptr(P["seed"]), nfe, n, _ffi.ptr(out), C.c_void_p(out.data_ptr() + 4 * B * D), _ffi.ptr(ws),
                 ws.numel(), _ffi.stream_ptr(dev)), "cfm_cnf_tc_field_f32")
+
+        P["field"] = field
+        P["field_split"] = lambda t, hi, lo, out, skip, n: field(t, None, out, n, hi, lo)
+
+    @staticmethod
+    def _grad_fields(mlp, P, B, D):
+        """The plan's field launchers for the gradient field of the action ``mlp`` in the tensor-core class: v into
+        ``out`` (row stride D, any 4-byte offset), from fp32 x or from the stage kernel's operand pair."""
+        L = _ffi.lib()
+        dev = P["dev"]
+        blob, gblob = mlp._grad_prepared(dev)
+        ws = _ffi.workspace(L.cfm_grad_tc_workspace_bytes(B, D, mlp.w), dev)
+        P["blob"], P["grad_blob"], P["grad_ws"] = blob, gblob, ws
+
+        def field(t, x, out, n, hi=None, lo=None):
+            _ffi.check(L.cfm_grad_tc_field_f32(
+                _ffi.ptr(blob), _ffi.ptr(gblob), _ffi.ptr(x), _ffi.ptr(hi), _ffi.ptr(lo), B, D, mlp.w, mlp.act,
+                _ffi.ptr(t), _ffi.ptr(out), _ffi.ptr(ws), ws.numel(), _ffi.stream_ptr(dev)), "cfm_grad_tc_field_f32")
 
         P["field"] = field
         P["field_split"] = lambda t, hi, lo, out, skip, n: field(t, None, out, n, hi, lo)

@@ -454,6 +454,45 @@ int cfm_cnf_tc_euler_init(cfm_cnf_tc_state* state, const float* z0, float* x, fl
 int cfm_cnf_tc_euler_step(cfm_cnf_tc_state* state, float* x, float* ll, const float* f, const float* div, void* x_hi,
                           void* x_lo, int batch, int dim, void* stream);
 
+/* ---- the action-matching gradient field of WIDE scalar actions, on the tensor cores ------------------------------
+ * replaces the field of torch_wrapper(GradModel(MLP(dim, out_dim=1, w, time_varying=True))) (action matching,
+ * examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb cells 10-11) for actions in the tensor-core
+ * class: v(t, x) = grad_x s(t, x) = W0x^T (D0 * W1^T (D1 * W2^T (D2 * W3[0, :]^T))), D_l = act'(pre_l).
+ * supported(): B >= 128, dim >= 32, dim and w multiples of 8, w >= 32 (cfm_mlp_tc_supported(batch, dim, w, dim)).
+ * Two blobs: mlp_prepared, the cfm_mlp_prepare blob of the action (out_dim = 1, time_varying = 1), and the blob of
+ * cfm_grad_tc_prepare, the K-major transposed fp16x3 pairs of W0x, W1 and W2 built from it (one launch; rebuild both
+ * when the weights change).  prepared_bytes() is 0 outside the class. */
+int cfm_grad_tc_supported(int batch, int dim, int w);
+size_t cfm_grad_tc_prepared_bytes(int dim, int w);
+int cfm_grad_tc_prepare(const void* mlp_prepared, int dim, int w, void* prepared, size_t prepared_bytes, void* stream);
+size_t cfm_grad_tc_workspace_bytes(int batch, int dim, int w);
+/* One field evaluation at (t = *t_dev, x) for `batch` rows: v [batch][dim] fp32, row stride dim, any 4-byte
+ * alignment.  x is given either as fp32 [batch][dim] (x_hi = x_lo = NULL; split here) or as its fp16x3 operand pair
+ * (x = NULL), as cfm_rk_stage_input writes it.  Six launches (seven with an fp32 x): three primal and three reverse
+ * GEMMs; no atomics, so the same call gives the same bits.  x, x_hi, x_lo, both blobs and the workspace 16-byte
+ * aligned; argument errors are reported before any CUDA call. */
+int cfm_grad_tc_field_f32(const void* mlp_prepared, const void* grad_prepared, const float* x, const void* x_hi,
+                          const void* x_lo, int batch, int dim, int w, int act, const float* t_dev, float* v,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* Euler driver state: step n evaluates the field at (t = t_span[n], x_n). */
+typedef struct cfm_grad_tc_state {
+  float* traj;            /* [n_span][batch][dim]                                             */
+  const float* t_span;    /* [n_span] fp32                                                    */
+  int32_t n;              /* next step                                                        */
+  int32_t n_steps;        /* n_span - 1                                                       */
+  float t;                /* t_span[n]: the time the evaluation of step n reads               */
+  uint32_t ticket;        /* CTAs of the running step that are done (0 between steps)         */
+} cfm_grad_tc_state;
+/* state <- (traj, t_span, n = 0, t = t_span[0]); x0 [batch][dim] -> x, traj[0] and (x_hi, x_lo), the fp16x3 operand
+ * split of x.  x0, x, x_hi, x_lo and traj 16-byte aligned. */
+int cfm_grad_tc_euler_init(cfm_grad_tc_state* state, const float* x0, float* x, void* x_hi, void* x_lo, float* traj,
+                           const float* t_span, int n_span, int batch, int dim, void* stream);
+/* Step n = state->n with h = (float)((double)t_span[n + 1] - (double)t_span[n]): x <- fmaf(h, v, x), traj[n + 1],
+ * (x_hi, x_lo); then n += 1, t = t_span[n + 1].  A step enqueued after the last one does nothing.  x, v, x_hi, x_lo
+ * 16-byte aligned. */
+int cfm_grad_tc_euler_step(cfm_grad_tc_state* state, float* x, const float* v, void* x_hi, void* x_lo, int batch,
+                           int dim, void* stream);
+
 /* ---- training step of small vector-field MLPs: the regression loss and all parameter gradients, ONE launch ------
  * replaces the three lines every training cell of the 2-D tutorials repeats per step
  * (examples/2D_tutorials/tutorial_training_8_gaussians_to_moons.ipynb raw lines 166-186, 310-330, 458-479, 602-623;
