@@ -13,10 +13,12 @@
 //   reverse       e W^T on the prepared K-major transposed pairs W2^T, W1^T ([w][w]) and W0x^T ([dim][w]): the first
 //                 two multiply by D and split (GradReverseEpi), the last writes v = acc 2^-k in fp32, row stride dim,
 //                 any 4-byte alignment: dopri5's stage slots are misaligned for odd B (GradOutEpi).
-// Scale of the reverse chain: the chain is linear in w3, so g2 carries ONE power of two 2^k with max|W3| 2^k in
-// [2^6, 2^7), taken from the forward blob's layer-3 scale (fixed when the blob is prepared); the last epilogue undoes it
-// exactly.  Small trained W3 then keeps the splits in fp16's normal range, and 2^7 leaves two layers of growth below
-// fp16's 65504 (DESIGN 3.18).  Scaling W3 by a power of two scales v by the same power, bit for bit.
+// Scale of the reverse chain: the chain is linear in w3, so g2 carries ONE power of two 2^k, fixed when the blob is
+// prepared and undone exactly by the last epilogue: the largest with max|W3| 2^k < 2^7 (from the forward blob's layer-3
+// scale; a small trained W3 then keeps the splits in fp16's normal range) whose bound of every split of the chain,
+// max|act'| max|W3| 2^k max(1, max|act'| C2, max|act'|^2 C2 C1) with C_l W_l's largest column abs-sum, stays at or
+// below fp16's 65504, so no saturating split clamps for any input (DESIGN 3.18).  Scaling W3 by a power of two scales v
+// by the same power, bit for bit.
 // No floating-point atomics: the same call gives the same bits.  The Euler driver's init and step kernels work like
 // cnf_tc.cu's: step index, time and the trajectory and span pointers live in a device struct, and a captured step
 // replays for the whole trajectory.
@@ -72,8 +74,6 @@ GradWs grad_ws(int batch, int dim, int w) {
 }
 
 // ---- prepare: W_l [w][cols] (stride lds, fp32, in the forward blob) -> (W_l s_l)^T split, [cols][w] -------------------
-// The scale of the reverse chain comes from the forward blob's layer-3 scale s_3, which puts max|W3| s_3 in
-// [2^13, 2^14): 2^k = s_3 2^-7 puts max|W3| 2^k in [2^6, 2^7).  Both factors are exact powers of two.
 struct TransposeJob {
   const float* src;
   int64_t lds;
@@ -83,19 +83,61 @@ struct TransposeJob {
 };
 struct TransposeJobs {
   TransposeJob j[3];
+  const float* w3;       // the forward blob's W3 [w], fp32
   const float* inv_ws3;  // the forward blob's 1 / s_3
   float* sc;             // out: {2^k, 2^-k / s_0}
 };
 
-// one 32 x 32 tile of layer blockIdx.z per CTA: coalesced reads along the inputs, coalesced writes along the units
-__global__ void __launch_bounds__(256) grad_transpose_split_kernel(const TransposeJobs jobs, int w) {
+// max|act'| over the activations the field takes: SELU's lambda alpha = 1.75809934..., rounded up (SiLU's is 1.0998)
+constexpr float kActPrimeMax = 1.7581f;
+constexpr int kTransposeThreads = 256;
+
+// The chain factors {2^k, 2^-k / s_0}, by one CTA of 256 threads.  The forward blob's layer-3 scale s_3 puts
+// max|W3| s_3 in [2^13, 2^14), so s_3 2^-7 is the largest 2^k with max|W3| 2^k < 2^7.  Each reverse layer l multiplies
+// |g| by at most max|act'| C_l, C_l = max_i sum_j |W_l[j, i]|, so every split sees at most
+//     max|act'| max|W3| 2^k max(1, max|act'| C2, max|act'|^2 C2 C1);
+// 2^k is lowered to the largest power of two that keeps this at or below 65504.  One thread per column adds its rows in
+// order and the maxima are exact, so the factors do not depend on the schedule.  Both rules scale with max|W3| by
+// exact powers of two, so W3 2^p still gives 2^-p 2^k.
+__device__ __forceinline__ void grad_chain_scale(const TransposeJobs& jobs, int w) {
+  __shared__ float red[3][kTransposeThreads / 32];
+  float c1 = 0.f, c2 = 0.f, m3 = 0.f;
+  for (int i = threadIdx.x; i < w; i += kTransposeThreads) {
+    float s1 = 0.f, s2 = 0.f;
+    for (int j = 0; j < w; ++j) {
+      s1 += fabsf(__ldg(jobs.j[1].src + (int64_t)j * jobs.j[1].lds + i));
+      s2 += fabsf(__ldg(jobs.j[2].src + (int64_t)j * jobs.j[2].lds + i));
+    }
+    c1 = fmaxf(c1, s1); c2 = fmaxf(c2, s2); m3 = fmaxf(m3, fabsf(__ldg(jobs.w3 + i)));
+  }
+  c1 = warp_max(c1); c2 = warp_max(c2); m3 = warp_max(m3);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) { red[0][wid] = c1; red[1][wid] = c2; red[2][wid] = m3; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int i = 1; i < kTransposeThreads / 32; ++i) {
+    c1 = fmaxf(c1, red[0][i]); c2 = fmaxf(c2, red[1][i]); m3 = fmaxf(m3, red[2][i]);
+  }
+  float k = 0x1p-7f / __ldg(jobs.inv_ws3);
+  const float b2 = kActPrimeMax * m3;            // |g2| / 2^k
+  const float b1 = b2 * (kActPrimeMax * c2);     // |g1| / 2^k
+  const float b0 = b1 * (kActPrimeMax * c1);     // |g0| / 2^k
+  const float peak = fmaxf(b2, fmaxf(b1, b0));
+  // the largest power of two <= 65504 / peak: the quotient's exponent bits (it is normal, or inf for a tiny peak)
+  if (peak > 0.f && peak <= 3.0e38f) k = fminf(k, __int_as_float(__float_as_int(65504.f / peak) & 0x7f800000));
+  jobs.sc[0] = k;
+  jobs.sc[1] = __ldg(jobs.j[0].inv_ws) / k;
+}
+
+// one 32 x 32 tile of layer blockIdx.z < 3 per CTA: coalesced reads along the inputs, coalesced writes along the units;
+// CTA (0, 0, 3) forms the chain factors (it reads only the forward blob, so it runs beside the tiles)
+__global__ void __launch_bounds__(kTransposeThreads) grad_transpose_split_kernel(const TransposeJobs jobs, int w) {
+  if (blockIdx.z == 3) {  // CTA-uniform
+    if ((blockIdx.x | blockIdx.y) == 0) grad_chain_scale(jobs, w);
+    return;
+  }
   __shared__ float tile[32][33];
   const TransposeJob& J = jobs.j[blockIdx.z];
-  if ((blockIdx.x | blockIdx.y | blockIdx.z | threadIdx.x) == 0) {
-    const float k = 0x1p-7f / __ldg(jobs.inv_ws3);
-    jobs.sc[0] = k;
-    jobs.sc[1] = __ldg(jobs.j[0].inv_ws) / k;
-  }
   const int u0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   if (c0 >= J.cols) return;  // CTA-uniform
   const float sc = 1.f / __ldg(J.inv_ws);  // exact: a power of two
@@ -299,13 +341,14 @@ extern "C" int cfm_grad_tc_prepare(const void* mlp_prepared, int dim, int w, voi
   char* dst = reinterpret_cast<char*>(prepared);
   const int64_t off[3] = {h.off_w0x, h.off_w1, h.off_w2}, lds[3] = {h.dimp, w, w};
   TransposeJobs J;
+  J.w3 = reinterpret_cast<const float*>(src + h.off_w3);
   J.inv_ws3 = W.inv_ws[3];
   J.sc = reinterpret_cast<float*>(dst + G.sc);
   for (int l = 0; l < 3; ++l)
     J.j[l] = TransposeJob{reinterpret_cast<const float*>(src + off[l]), lds[l], l ? w : dim, W.inv_ws[l],
                           reinterpret_cast<__half*>(dst + G.wth[l]), reinterpret_cast<__half*>(dst + G.wtl[l])};
-  const dim3 grid((w + 31) / 32, (std::max(dim, w) + 31) / 32, 3);
-  grad_transpose_split_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(J, w);
+  const dim3 grid((w + 31) / 32, (std::max(dim, w) + 31) / 32, 4);  // z = 3: the chain factors' CTA
+  grad_transpose_split_kernel<<<grid, kTransposeThreads, 0, (cudaStream_t)stream>>>(J, w);
   note_launches(1);
   CFM_CUDA_OK(cudaGetLastError());
   return CFM_OK;

@@ -19,9 +19,14 @@
   those rows; the tests count them and bound their share.
 * ``lipschitz``: a Lipschitz bound of v in x for the trajectory bounds (the three terms of the product rule through
   D0, D1 and D2, with spectral norms).
+* ``layer_scales``: the powers of two of both prepared blobs, restated in float32 from gemm_h3.cuh's h3_pow2_scale and
+  grad_tc.cu's chain rule: s_0..s_3 and the chain factors {2^k, 2^-k / s_0}.  ``chain_peaks``: the largest |g_l 2^k|
+  the three saturating splits of the reverse chain see, in float64.  ``grad_blob``: the prepared gradient blob, byte
+  for byte.
 """
 import math
 
+import numpy as np
 import torch
 
 EPS_GEMM = 1e-6
@@ -104,3 +109,107 @@ def lipschitz(state, act, dim):
     lp = [N[0], N[0] * N[1] * slope, N[0] * N[1] * N[2] * slope ** 2]  # Lipschitz bounds of pre_0, pre_1, pre_2
     # the term of D_l: every weight norm, the two other D's at most slope each, and max|act''| Lip(pre_l)
     return n3 * math.prod(N) * slope ** 2 * d2max * sum(lp)
+
+
+# ---- the scales of the prepared blobs (float32, as the kernels form them) ---------------------------------------------
+FP16_MAX = 65504.0
+ACT_PRIME_MAX = np.float32(1.7581)  # grad_tc.cu's kActPrimeMax: >= max|act'| of SELU (lambda alpha) and SiLU (1.0998)
+
+
+def _ilogb(v):
+    return int(np.frexp(np.float32(v))[1]) - 1
+
+
+def pow2_scale(am):
+    """gemm_h3.cuh's h3_pow2_scale: 2^(13 - ilogb(am)), the exponent clamped to [-100, 100]; 1 for a zero or non-finite
+    am."""
+    am = np.float32(am)
+    if not (am > 0 and am < np.float32(3.0e38)):
+        return np.float32(1.0)
+    return np.float32(2.0 ** max(-100, min(100, 13 - _ilogb(am))))
+
+
+def _weights32(state, dim):
+    """W0x, W1, W2, W3 as float32 NumPy arrays (W0x = W0[:, :dim])."""
+    W = [state[f"net.{li}.weight"].detach().float().cpu().numpy() for li in (0, 2, 4, 6)]
+    return [np.ascontiguousarray(W[0][:, :dim])] + W[1:]
+
+
+def col_abs_sum_max(W):
+    """max_i sum_j |W[j, i]| in float32, rows added in order (one thread per column, as grad_chain_scale)."""
+    acc = np.zeros(W.shape[1], np.float32)
+    for j in range(W.shape[0]):
+        acc += np.abs(W[j])
+    return np.float32(acc.max())
+
+
+def layer_scales(state, dim, chain_bound=True):
+    """(s_0..s_3, {2^k, 2^-k / s_0}) as cfm_mlp_prepare and cfm_grad_tc_prepare form them.  2^k is the largest power of
+    two with max|W3| 2^k < 2^7 (2^k = s_3 2^-7) and, with ``chain_bound``, with every split of the reverse chain bounded
+    by 65504: max|act'| max|W3| 2^k max(1, max|act'| C2, max|act'|^2 C2 C1) <= 65504, C_l the largest column
+    abs-sum of W_l.  ``chain_bound=False`` is the W3-only rule."""
+    W = _weights32(state, dim)
+    s = [pow2_scale(np.abs(Wl).max()) for Wl in W]
+    k = np.float32(2.0 ** -7) / (np.float32(1) / s[3])
+    if chain_bound:
+        A = ACT_PRIME_MAX
+        m3 = np.float32(np.abs(W[3]).max())
+        c1, c2 = col_abs_sum_max(W[1]), col_abs_sum_max(W[2])
+        b2 = A * m3
+        b1 = b2 * (A * c2)
+        b0 = b1 * (A * c1)
+        peak = max(b2, b1, b0)
+        if peak > 0 and peak <= np.float32(3.0e38):
+            with np.errstate(over="ignore"):
+                q = np.float32(FP16_MAX) / peak
+                lim = np.float32(np.inf) if np.isinf(q) else np.ldexp(np.float32(1), _ilogb(q)).astype(np.float32)
+            k = min(k, lim)
+    return s, (np.float32(k), (np.float32(1) / s[0]) / np.float32(k))
+
+
+def chain_peaks(state, t, x, act, sk=None):
+    """(max|g2 2^k|, max|g1 2^k|, max|g0 2^k|) in float64: the values the three saturating splits of the reverse chain
+    see; 2^k from ``layer_scales`` unless given."""
+    _, d1, _, _ = _acts(act)
+    W, _ = _params(state, x.device)
+    if sk is None:
+        sk = float(layer_scales(state, x.shape[1])[1][0])
+    D = [d1(pre) for pre, _ in _forward(state, t, x, act)]
+    g2 = D[2] * W[3][0] * sk
+    g1 = D[1] * (g2 @ W[2])
+    g0 = D[0] * (g1 @ W[1])
+    return float(g2.abs().max()), float(g1.abs().max()), float(g0.abs().max())
+
+
+def activation_peak(state, t, x, act):
+    """max|a_l| over the two activations the forward splits (layers 0 and 1) and x itself."""
+    f_act = _acts(act)[0]
+    pre = _forward(state, t, x, act)
+    return max(float(x.abs().max()), *(float(f_act(p).abs().max()) for p, _ in pre[:2]))
+
+
+def grad_blob(state, dim, w):
+    """(bytes, regions): the prepared gradient blob of cfm_grad_tc_prepare as a uint8 array, and its defined regions
+    [(name, offset, nbytes)] (the 1024-byte alignment gaps between them are not written).  GradBlob's layout: the chain
+    factors {2^k, 2^-k / s_0} first, then per layer l = 0, 1, 2 the K-major (W_l s_l)^T [cols][w] split as hi =
+    fp16_rn(v), lo = fp16_rn((v - hi) 2^11) (split_h3; NumPy's float16 cast rounds to nearest even like
+    __float2half_rn)."""
+    W = _weights32(state, dim)
+    s, sc = layer_scales(state, dim)
+
+    def align(n):
+        return (n + 1023) // 1024 * 1024
+    regions, o = [], 0
+    parts = [("sc", np.array(sc, np.float32).view(np.uint8))]
+    for li in range(3):
+        v = np.ascontiguousarray((W[li] * s[li]).T.astype(np.float32))
+        hi = v.astype(np.float16)
+        lo = ((v - hi.astype(np.float32)) * np.float32(2048)).astype(np.float16)
+        parts += [(f"wth{li}", hi.view(np.uint8).ravel()), (f"wtl{li}", lo.view(np.uint8).ravel())]
+    for name, p in parts:
+        regions.append((name, o, p.size))
+        o += align(p.size)
+    out = np.zeros(o, np.uint8)
+    for (name, off, n), (_, p) in zip(regions, parts):
+        out[off:off + n] = p
+    return out, regions

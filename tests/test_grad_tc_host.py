@@ -220,3 +220,116 @@ def test_other_refusals_stay():
         node._grad_trajectory_on(action, torch.zeros(256, 64), torch.linspace(0, 1, 3), torch.device("cpu"))
     with pytest.raises(_ffi.CfmLibraryError, match="needs CUDA inputs"):  # in the class: no CPU fallback
         _node(action, solver="euler").trajectory(torch.zeros(256, 64), torch.linspace(0, 1, 3))
+
+
+# ---- the scales of the prepared blobs ---------------------------------------------------------------------------------
+def _scaled_state(dim, w, factors, act="selu", seed=gc.LAYER_SCALE_SEED):
+    return {k: v.detach() for k, v in gc.scaled_action(dim, w, seed, factors, act).state_dict().items()}
+
+
+def test_scale_rules_match_the_sources():
+    """grad_tc_oracle.layer_scales restates h3_pow2_scale and the chain rule of grad_tc.cu's grad_chain_scale."""
+    h3 = open(os.path.join(CSRC, "gemm_h3.cuh")).read()
+    body = re.search(r"float h3_pow2_scale\(float am\) \{(.*?)\n\}", h3, re.S).group(1)
+    assert "if (am > 0.f && am < 3.0e38f)" in body and "e = max(-100, min(100, 13 - e));" in body
+    assert "int e = ilogbf(am);" in body and "sc = scalbnf(1.f, e);" in body
+    src = open(os.path.join(CSRC, "grad_tc.cu")).read()
+    A = float(re.search(r"constexpr float kActPrimeMax = ([\d.]+)f;", src).group(1))
+    assert go.ACT_PRIME_MAX == go.np.float32(A)
+    assert A >= go.SELU_L * go.SELU_A and A >= 1.0998  # SELU's lambda alpha and SiLU's max act'
+    body = re.search(r"void grad_chain_scale\((.*?)\n\}", src, re.S).group(1)
+    for line in ["s1 += fabsf(__ldg(jobs.j[1].src + (int64_t)j * jobs.j[1].lds + i));",
+                 "s2 += fabsf(__ldg(jobs.j[2].src + (int64_t)j * jobs.j[2].lds + i));",
+                 "float k = 0x1p-7f / __ldg(jobs.inv_ws3);",
+                 "const float b2 = kActPrimeMax * m3;", "const float b1 = b2 * (kActPrimeMax * c2);",
+                 "const float b0 = b1 * (kActPrimeMax * c1);", "const float peak = fmaxf(b2, fmaxf(b1, b0));",
+                 "if (peak > 0.f && peak <= 3.0e38f) k = fminf(k, __int_as_float(__float_as_int(65504.f / peak) & "
+                 "0x7f800000));",
+                 "jobs.sc[0] = k;", "jobs.sc[1] = __ldg(jobs.j[0].inv_ws) / k;"]:
+        assert line in body, line
+    # the transpose scales each layer by its own s_l, and the epilogues undo layer 2's, then layer 1's
+    assert "const float sc = 1.f / __ldg(J.inv_ws);" in src
+    assert "if ((blockIdx.x | blockIdx.y) == 0) grad_chain_scale(jobs, w);" in src
+    assert "J.inv_ws3 = W.inv_ws[3];" in src
+    assert "GradReverseEpi r2{W.inv_ws[2]," in src and "GradReverseEpi r1{W.inv_ws[1]," in src
+    assert "GradSeedEpi se{F(boff[2]), W.inv_ws[2]," in src and "GradOutEpi r0{sc + 1," in src
+
+
+def test_pow2_scale_restatement():
+    assert go.pow2_scale(0.0) == 1 and go.pow2_scale(float("inf")) == 1 and go.pow2_scale(float("nan")) == 1
+    assert go.pow2_scale(1.0) == 2.0 ** 13 and go.pow2_scale(1.5) == 2.0 ** 13 and go.pow2_scale(2.0) == 2.0 ** 12
+    assert go.pow2_scale(2.0 ** -110) == 2.0 ** 100 and go.pow2_scale(2.0 ** 120) == 2.0 ** -100
+    assert go.pow2_scale(2.0 ** -140) == 2.0 ** 100  # a float32 subnormal
+
+
+@pytest.mark.parametrize("factors", gc.LAYER_SCALE_SETS)
+@pytest.mark.parametrize("B,dim,w", gc.LAYER_SCALE_SHAPES)
+def test_layer_scale_sets_give_distinct_scales(B, dim, w, factors):
+    s, (k, k0) = go.layer_scales(_scaled_state(dim, w, factors), dim)
+    vals = [float(v) for v in s] + [float(k)]
+    assert len(set(vals)) == 5, vals
+    assert float(k0) == 1 / (float(s[0]) * float(k))
+
+
+def test_layer_scale_sets_rank_each_hidden_layer_first_and_last():
+    hidden = [f[:3] for f in gc.LAYER_SCALE_SETS]
+    assert {h.index(max(h)) for h in hidden} == {0, 1, 2} and {h.index(min(h)) for h in hidden} == {0, 1, 2}
+    assert all(f[3] not in f[:3] for f in gc.LAYER_SCALE_SETS)
+
+
+@pytest.mark.parametrize("act,factors,frac", gc.RANGE_CASES)
+def test_range_cases_reach_their_fraction(act, factors, frac):
+    """Under the W3-only rule 2^k = s_3 2^-7 the chain peaks at the claimed fraction of 65504; under the chain bound no
+    split passes 65504; the forward activations stay far below it."""
+    B, dim, w = gc.RANGE_SHAPE
+    state = _scaled_state(dim, w, factors, act, seed=7)
+    x = gc.range_input(B, dim).double()
+    _, (k_w3, _) = go.layer_scales(state, dim, chain_bound=False)
+    got = max(go.chain_peaks(state, 0.3, x, act, sk=float(k_w3))) / go.FP16_MAX
+    assert abs(got - frac) <= 0.01 * frac, (got, frac)
+    assert max(go.chain_peaks(state, 0.3, x, act)) <= go.FP16_MAX
+    assert go.activation_peak(state, 0.3, x, act) <= 0.1 * go.FP16_MAX
+
+
+def test_chain_bound_keeps_the_default_action_and_lowers_the_scaled_ones():
+    """At the default-initialised MNIST action the bound leaves 2^k = s_3 2^-7; W0..W2 x 3 and x 11 lower it by 2^3 and
+    2^7."""
+    dim, w = 784, 256
+    for f, drop in ((1.0, 0), (3.0, 3), (11.0, 7)):
+        state = _scaled_state(dim, w, (f, f, f, 1.0), seed=7)
+        k_w3 = go.layer_scales(state, dim, chain_bound=False)[1][0]
+        k = go.layer_scales(state, dim)[1][0]
+        assert k_w3 / k == 2.0 ** drop, (f, k_w3, k)
+
+
+def test_chain_factor_is_linear_in_w3():
+    dim, w = 72, 136
+    state = _scaled_state(dim, w, (20.0, 20.0, 20.0, 1.0))
+    k = float(go.layer_scales(state, dim)[1][0])
+    for p in gc.W3_POWERS:
+        st = dict(state)
+        st["net.6.weight"] = state["net.6.weight"] * 2.0 ** p
+        assert float(go.layer_scales(st, dim)[1][0]) == k * 2.0 ** -p, p
+
+
+@pytest.mark.parametrize("dim,w,factors", [(784, 256, (1.0,) * 4), (32, 40, (1.0,) * 4), (264, 264, (1.0,) * 4),
+                                           (72, 136, gc.LAYER_SCALE_SETS[1])])
+def test_grad_blob_matches_a_float64_transpose(dim, w, factors):
+    np = go.np
+    state = _scaled_state(dim, w, factors)
+    blob, regions = go.grad_blob(state, dim, w)
+    s, sc = go.layer_scales(state, dim)
+    r = {name: (off, n) for name, off, n in regions}
+    assert r["sc"] == (0, 8) and all(off % 1024 == 0 for off, _ in r.values())
+    assert blob[:8].view(np.float32).tolist() == [float(sc[0]), float(sc[1])]
+    W = go._weights32(state, dim)
+    for li in range(3):
+        ref = W[li].astype(np.float64).T * float(s[li])
+        rows = dim if li == 0 else w
+        got = []
+        for part in ("wth", "wtl"):
+            off, n = r[f"{part}{li}"]
+            assert n == rows * w * 2
+            got.append(blob[off:off + n].view(np.float16).astype(np.float64).reshape(rows, w))
+        val = got[0] + got[1] * 2.0 ** -11
+        assert np.all(np.abs(val - ref) <= 2.0 ** -22 * np.abs(ref) + 2.0 ** -35), li
